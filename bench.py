@@ -1,4 +1,5 @@
-"""bench.py -- env-steps/s of one full BatchPolopt iteration (rollout + process_samples + policy update) on B200.
+"""bench.py -- env-steps/s of one full BatchPolopt iteration (rollout + process_samples + policy update) on one GPU
+(written for the H100).
 
 Workload (BASELINE.json configs[1]): CartPoleEnv, 65 536 lanes per GPU, horizon 200, VPG + LinearFeatureBaseline,
 GaussianMLPPolicy(32,32).  One "step" = one training iteration = N*T env steps.
@@ -8,6 +9,8 @@ GaussianMLPPolicy(32,32).  One "step" = one training iteration = N*T env steps.
            read back), host<->device copies inside the timed region.
   --impl reference : the reference's CPU sampler structure (oracle/cpu_sampler.py: per-path Python rollouts in a
            process pool over all host cores + NumPy update) on a bounded sample of the same workload.
+  --dump-outputs DIR : after the timed steps, DIR/<name>.npy holds what the last timed iteration computed (see
+           dump_outputs); the inputs are seeded, so two builds run with the same arguments can be compared array by array.
 """
 import argparse
 import json
@@ -56,8 +59,45 @@ def make_env(name):
     raise ValueError(name)
 
 
+DUMP_LANES = 512                # lanes in the fixed, seeded sample of the trajectory arrays written by --dump-outputs
+DUMP_BYTES = 64 * 1024 * 1024   # upper bound of everything --dump-outputs writes
+
+
+def dump_outputs(out_dir, algo, policy, baseline):
+    """Write what the last iteration handed its caller: the updated policy parameters, the fitted baseline coefficients
+    and, for a fixed seeded sample of at most DUMP_LANES lanes and (where the horizon would exceed DUMP_BYTES) of time
+    steps, the trajectory arrays with their advantages and returns ([dim][steps][lanes] / [steps][lanes]).  Float32
+    device buffers are written as float32, the float64 ones as float64."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    b = algo.sampler.batch
+    arrays = dict(policy_params=np.asarray(policy.get_param_values(), dtype=np.float64))
+    coeffs = baseline.get_param_values()
+    if coeffs is not None:
+        arrays["baseline_coeffs"] = np.asarray(coeffs, dtype=np.float64)
+    lanes = np.sort(np.random.RandomState(0).choice(b.N, min(DUMP_LANES, b.N), replace=False))
+    per_step = 4 * (b.O + 2 * b.A + 3) * len(lanes) + 8      # bytes of one sampled step over the batch arrays
+    budget = DUMP_BYTES - 8 * (len(lanes) + sum(v.size for v in arrays.values())) - 64 * 1024
+    steps = np.arange(b.T)
+    if b.T * per_step > budget:
+        steps = np.sort(np.random.RandomState(1).choice(b.T, budget // per_step, replace=False))
+    arrays["sample_lanes"] = lanes.astype(np.float64)
+    arrays["sample_steps"] = steps.astype(np.float64)
+    li = torch.as_tensor(lanes, device=b.obs.device)
+    ti = torch.as_tensor(steps, device=b.obs.device)
+    for k in ("obs", "act", "mean", "rew", "adv", "ret"):
+        v = getattr(b, k).index_select(-1, li).index_select(-2, ti)
+        arrays["batch_" + k] = v.cpu().numpy().astype(np.float32)
+    total = sum(v.nbytes for v in arrays.values())
+    assert total <= DUMP_BYTES, "dump of %d bytes exceeds %d" % (total, DUMP_BYTES)
+    for name, v in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), v)
+
+
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -107,7 +147,7 @@ def measured_peaks():
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, sustained copy)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def cpu_arm(workload, steps, warmup, cores=None, sample_steps=None, seconds_budget=20.0):
@@ -153,6 +193,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the short TRPO workloads reported under extra.workloads")
     ap.add_argument("--cpu-seconds", type=float, default=15.0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed iteration's outputs as DIR/<name>.npy")
     ap.add_argument("--cpu-arm-json", action="store_true", help=argparse.SUPPRESS)   # internal: CPU leg in a clean process
     args = ap.parse_args()
     assert args.warmup >= 0 and args.steps >= 1
@@ -253,6 +295,8 @@ def main():
     k0, c0, x0 = L.kernel_launches(), comm.n_collectives, comm.n_peer_exchanges
     ms_dev = run(algo, policy, args.steps, itr, False)
     launches = (L.kernel_launches() - k0) / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, algo, policy, baseline)
     collectives = (comm.n_collectives - c0) / args.steps            # NCCL collectives on the iteration's critical path
     peer_exchanges = (comm.n_peer_exchanges - x0) / args.steps      # peer-memory exchanges (fused or stand-alone kernels)
     itr += args.steps
@@ -317,7 +361,7 @@ def main():
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) / reps
 
-    # FP32 roofline of this box, measured here: 16 independent fma.rn.f32x2 chains per thread, no memory traffic
+    # FP32 roofline of this GPU, measured here: 16 independent float2 FMA chains per thread, no memory traffic
     sink = torch.zeros(4, dtype=torch.float32, device=dev)
     import ctypes
     fma = ctypes.c_longlong(0)
@@ -365,23 +409,14 @@ def main():
         v["frac"] = (v["GBps"] / hbm_peak) if v["bound"] == "hbm" else (v["TFLOPs"] / fp32_peak)
         v["share_of_step"] = v["ms"] * v["per_iter"] / (ms_dev / args.steps)
     dom = max(kern, key=lambda k: kern[k]["ms"] * kern[k]["per_iter"])
-    # dram bytes per launch from the ncu --set full capture of the shipped build (profiles/r02_traffic.json, written by
-    # scripts/ncu_traffic.py from the committed capture); only quoted for the profiled geometry
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    if os.path.exists(tpath) and args.lanes is None and args.horizon is None:
-        try:
-            traffic = json.load(open(tpath)).get(args.workload, {}).get(dom)
-        except Exception:
-            traffic = None
     kd = kern[dom]
     if kd["bound"] == "hbm":
         roofline = dict(bound="hbm", kernel=dom, achieved=kd["GBps"], peak=hbm_peak, unit="GB/s", frac=kd["frac"],
-                        traffic=traffic, peak_source=hbm_src)
+                        peak_source=hbm_src)
     else:
         roofline = dict(bound="fp32_issue", kernel=dom, achieved=kd["TFLOPs"], peak=fp32_peak, unit="TFLOP/s",
-                        frac=kd["frac"], traffic=traffic,
-                        peak_source="measured in this run: b200rl_bench_ffma2 (independent fma.rn.f32x2 chains, no memory)",
+                        frac=kd["frac"],
+                        peak_source="measured in this run: b200rl_bench_ffma2 (independent FMA chains, no memory)",
                         algorithmic_flops_per_launch=kd["flops"], algorithmic_bytes_per_launch=kd["bytes"],
                         hbm_GBps=kd["GBps"], hbm_frac=kd["GBps"] / hbm_peak,
                         note="the policy passes are bound by FP32 / instruction issue (%.0f flop per byte), not by HBM; "
@@ -422,7 +457,7 @@ def main():
         config=dict(workload=args.workload, env=env_name, algo=algo_name, lanes_per_gpu=lanes, horizon=T,
                     hidden=[hidden, hidden], samples_per_step=steps_per_iter, parallelism="lanes sharded x%d" % world,
                     whole_paths=bool(algo.whole_paths), valid_samples_per_step=n_valid,
-                    l2="trajectory buffers (%.0f MB/GPU) exceed the 126 MB L2" % (b.B * (alg_bytes + 14) / 1e6)),
+                    l2="trajectory buffers (%.0f MB/GPU) exceed the 50 MB L2" % (b.B * (alg_bytes + 14) / 1e6)),
         e2e=dict(value=e2e_value, unit="env-steps/s", ms_per_step=ms_e2e / args.steps,
                  h2d_bytes_per_step=8 * P_, d2h_bytes_per_step=8 * P_ + d2h_stats),
         gpu_launches=launches, collectives_per_step=collectives, peer_exchanges_per_step=peer_exchanges,

@@ -1,5 +1,5 @@
 /*
- * b200rl.h -- C ABI of libb200rl.so: the B200-native (sm_100a) implementation of rllab's
+ * b200rl.h -- C ABI of libb200rl.so: the H100-native (sm_90a) implementation of rllab's
  * data-parallel hot path (lock-step lane rollout, process_samples, VPG / TRPO update).
  *
  * The reference (rll/rllab @ ba78e4c) has NO native boundary on this path: the path is pure Python over
@@ -69,7 +69,7 @@ int b200rl_version(void);
 /* Number of CUDA kernels this library has launched in this process (bench.py reports the per-step delta). */
 unsigned long long b200rl_kernel_launches(void);
 /* FP32 roofline microbenchmark (no memory traffic): queues one kernel of num_SMs*8 blocks x 256 threads, each thread
- * running iters x 16 independent packed fma.rn.f32x2; *fma_out_host = scalar FMAs executed.  The caller times it (CUDA
+ * running iters x 16 independent float2 FMA chains; *fma_out_host = scalar FMAs executed.  The caller times it (CUDA
  * events) -- bench.py reports the policy passes against this measured FP32 peak. */
 int b200rl_bench_ffma2(int iters, float* sink, long long* fma_out_host, void* stream);
 /* SM count of the current device (grid sizing helper for callers that size workspaces). */
@@ -161,7 +161,7 @@ int b200rl_lfb_solve(int obs_dim, const double* gram, double reg_coeff, double* 
  * (sums_out[2] of b200rl_process_samples): pass scale = 1 and count = &sums[2] for the mean over the valid samples of
  * all ranks without reading the count back to the host.
  * Arithmetic of the three update passes (loss_kl, grad, fvp): float32 per sample, float32 sums inside one 128-sample
- * tile, float64 above.  (32,32) nets: every pass runs its dense layers on the tcgen05 tensor cores with the three-pass
+ * tile, float64 above.  (32,32) nets: every pass runs its dense layers on the wgmma tensor cores with the three-pass
  * TF32 split (float32-grade, 4e-7 of the output scale); (64,64) nets: grad and fvp (with h_cache) likewise, loss_kl on
  * the FP32 pipe in the rollout's summation order (ratio exactly 1 at theta_old).  While b200rl_peer_fuse_updates(1) is in
  * effect the outputs are reduced over all ranks of the bound peer communicator inside the pass. */

@@ -23,18 +23,16 @@ int cuda_fail(cudaError_t e, const char* what) {
 int num_sms() {
   static int cached[64] = {0};       // per device: a process may drive several GPUs
   int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (cached[dev & 63] > 0) return cached[dev & 63];
-  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) return 148;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) return 132;
   cached[dev & 63] = sms;
   return sms;
 }
 
 // out[k] = op over blocks of partial[b][k].  32 outputs x FIN_SLICES block-slices per CTA: each slice walks every
 // FIN_SLICES-th block (coalesced 256 B rows, 4 loads in flight), the slices are combined through shared memory in fixed
-// order, so the result is deterministic and the dependent-add chain is nblocks/FIN_SLICES long instead of nblocks (the
-// one-thread-per-output version cost ~56 us per call -- profiles/r01c; 8 slices still 40 us on the 2 048 partials of
-// process_samples -- profiles/r02a).
+// order, so the result is deterministic and the dependent-add chain is nblocks/FIN_SLICES long instead of nblocks.
 constexpr int FIN_SLICES = 32, FIN_THREADS = 32 * FIN_SLICES;
 template <bool IS_MAX>
 __global__ void __launch_bounds__(FIN_THREADS) finalize_kernel(const double* __restrict__ partial, int nblocks, int K,
@@ -185,9 +183,9 @@ int launch_finalize_update(const FinArgs& f, cudaStream_t s) {
   return 0;
 }
 
-// FP32 issue-rate microbenchmark: 16 independent packed-FMA chains per thread, no memory traffic.  bench.py times it with
-// CUDA events to obtain the FP32 roofline of THIS box (MEASURED_PEAKS.json carries HBM and bf16 tensor peaks only): the
-// policy passes are bound by FP32 / instruction issue, not by HBM.
+// FP32 issue-rate microbenchmark: 16 independent float2 FMA chains per thread (two scalar FFMAs each on sm_90, one
+// packed FFMA2 where the GPU has it), no memory traffic.  bench.py times it with CUDA events to obtain the FP32 roofline
+// of the GPU it runs on: the policy passes are bound by FP32 / instruction issue, not by HBM.
 __global__ void __launch_bounds__(256) peak_ffma2_kernel(int iters, float seed, float* __restrict__ sink) {
   float2 acc[16];
 #pragma unroll

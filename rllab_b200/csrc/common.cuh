@@ -1,4 +1,4 @@
-// Shared device/host helpers for libb200rl (sm_100a only).
+// Shared device/host helpers for libb200rl (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -53,7 +53,7 @@ int num_sms();
   } while (0)
 
 // partial-reduction workspace geometry: every reduction kernel uses at most MAX_PARTIAL_BLOCKS blocks and
-// writes [block][K] float64 partials; K <= MAX_PARTIAL_K.
+// writes [block][K] float64 partials; K <= MAX_PARTIAL_K.  (8 blocks per SM on GPUs of up to 148 SMs.)
 constexpr int MAX_PARTIAL_BLOCKS = 148 * 8;
 constexpr int MAX_PARTIAL_K = 8192;
 
@@ -118,8 +118,7 @@ __device__ __forceinline__ void noise4(int kind, uint32_t seed, uint32_t iter, i
 // theta_old): 1 - 2 / (2^(2 log2(e) x) + 1) with MUFU.EX2 + MUFU.RCP -- 5 instructions instead of tanhf's ~14 (tanhf was
 // 39 % of the rollout's instruction stream); saturates correctly (+inf -> 1, 0 -> -1); absolute error <= ~4e-7 (relative
 // accuracy is lost near 0, which the activations do not need: policy mean off by 8e-7 of its scale against a test
-// tolerance of 2e-5).  A/B on a B200 (round 2, cfg2): rollout 1.45 -> 1.18 ms, loss/KL 1.25 -> 1.04 ms, gradient
-// 3.41 -> 3.23 ms with the full parity suite unchanged.
+// tolerance of 2e-5).
 __device__ __forceinline__ float tanh_f(float x) {
   float e, r;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * 2.885390081777927f));

@@ -4,7 +4,7 @@
 // Canonical summation order (shared by the thread-per-lane rollout and the warp-per-sample update kernels so
 // that mean(theta_old) is bit-identical in both, i.e. the likelihood ratio at theta_old is exactly 1):
 //   dot(in, w, n, bias): s0 = bias, s1 = 0; s0 += in[i]*w[i] for even i, s1 += in[i]*w[i] for odd i (fma, ascending
-//   i); result = s0 + s1.   On sm_100 the even/odd pair maps onto one packed FFMA2 (fma.rn.f32x2).
+//   i); result = s0 + s1.   ffma2() computes an even/odd pair (two FFMAs on sm_90).
 #pragma once
 #include "common.cuh"
 

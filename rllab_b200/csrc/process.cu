@@ -106,7 +106,7 @@ __global__ void __launch_bounds__(PRED_THREADS) lfb_predict_kernel(int O_rt, lon
   for (long long i = done + gt; i < B; i += stride) base[i] = (float)lfb_predict<OT>(obs, (size_t)B, (size_t)i, O, tstep[i], sw);
 }
 
-// 14 warps of 32 lanes per SM hold cfg2's 65 536 lanes in ONE wave (148 x 14 x 32 = 66 304).  The inputs of the next
+// 14 warps of 32 lanes per SM hold cfg2's 65 536 lanes in about one wave (132 x 14 x 32 = 59 136).  The inputs of the next
 // SC_AHEAD chunks of SC_CH steps are staged through a warp-private shared-memory ring with cp.async (LDGSTS, 16 B per
 // lane, 22 lanes per step row: 128 B rew + 128 B base + 64 B tstep + 32 B flags), so the look-ahead (32 steps = 11 KB per
 // warp, 154 KB per SM in flight) does not cost registers; the scan reads its step back with four conflict-free LDS.

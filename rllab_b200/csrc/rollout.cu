@@ -65,11 +65,9 @@ struct RolloutArgs {
 };
 
 // Policy weights of the 32-wide rollout through the CONSTANT bank: with theta in a __constant__ array the dense layers
-// compile to `LDCU.128 UR, c[...]` (uniform datapath, one load per warp) + `FFMA2 R, R.F32, UR.F32x2, R` -- the weight
-// pair is a uniform-register operand -- instead of LDS.128 + vector registers (the fully unrolled 32-wide layers index
-// the weights with compile-time offsets).  A/B on a B200 (round 2, cfg2, together with the 5-instruction tanh): rollout
-// 1.18 -> 1.00 ms, 92 registers.  The same change LOSES in the thread-per-sample update kernels (tile gradient 3.2 ->
-// 4.4 ms: its staging wants the registers), which therefore keep theta in shared memory.  theta is refreshed by one
+// compile to FFMAs with a constant-bank operand (one load per warp, no LSU traffic) instead of LDS.128 + vector registers
+// (the fully unrolled 32-wide layers index the weights with compile-time offsets).  The thread-per-sample update
+// kernels keep theta in shared memory: their staging wants the registers.  theta is refreshed by one
 // stream-ordered device-to-device cudaMemcpyToSymbolAsync (<= 7 KB) per rollout.
 constexpr int ROLLOUT_CONST_MAXP = 2048;     // >= P of the largest 32-wide net (Hopper obs 20: 1 830)
 __constant__ __align__(16) float c_theta[ROLLOUT_CONST_MAXP];

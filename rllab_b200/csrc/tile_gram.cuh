@@ -1,4 +1,4 @@
-// Gram phase of the 32-wide update kernels (update_tile.cu: FP32 layer chain; update_umma32.cu: tcgen05 layer chain): the
+// Gram phase of the 32-wide update kernels (update_tile.cu: FP32 layer chain; update_umma32.cu: tensor-core layer chain): the
 // weight gradients as Gram products over one 128-sample tile staged feature-major in shared memory,
 //     dW0 = X^T D1, db0 = 1^T D1, dW1 = H1^T D2, db1 = 1^T D2, dWout = H2^T DM, dbout = 1^T DM, dlog_std = 1^T DL,
 // accumulated by the 128 threads of the CTA: dW1 (32 x 32 outputs, the bulk) in 4x4 register tiles, rows interleaved by 8
@@ -48,7 +48,7 @@ __device__ __forceinline__ void tile_dist_init(TileDist& D, const float* log_std
 //   part B  dW0[o, :] for o = warp, warp + 4, ... and db0 (warp 3)                     -- reads X, D1
 // Every small output is spread over the four warps: with one warp per output group (the first layout) warp 0 carried
 // dW1 + all of dW0 -- 2.7x the work of the others for obs_dim 13 -- and set the length of the phase.
-// PACKED: dW1 with packed FFMA2 (two samples per instruction, even / odd partial sums).
+// PACKED: dW1 with float2 even / odd partial sums (two samples per ffma2()).
 template <class N, int RX, int RH1, int RH2, int RD1, int RD2, int RDM, int LD, bool PACKED = false>
 struct TileGram {
   static constexpr int O = N::O, H = 32, A = N::A, TILE = 128;

@@ -128,7 +128,7 @@ int b200rl_loss_kl(int loss_kind, const float* params_f32, int obs_dim, int h1, 
   int grid = 0;
 #ifndef B200RL_AB_TILE32
   if (h1 == 32 && h2 == 32) {
-    // 32-wide nets: forward-only mode of the tcgen05 kernel (update_umma32.cu) -- the same forward, instruction for
+    // 32-wide nets: forward-only mode of the tensor-core kernel (update_umma32.cu) -- the same forward, instruction for
     // instruction, as the gradient pass, so (loss, KL) of the two passes agree bit for bit at equal theta
     int P = 0, ols = 0;
     int rc = update_umma32_launch(MODE_LOSS, obs_dim, act_dim, a, &grid, &P, &ols, st);
@@ -196,8 +196,8 @@ int b200rl_fvp(const float* params_f32, int obs_dim, int h1, int h2, int act_dim
   fill_args(a, params_f32, min_std, B, obs, nullptr, nullptr, nullptr, nullptr, B200RL_LOSS_TRPO, flags, ws);
   a.xvec = x; a.h_cache = const_cast<float*>(h_cache); a.tile_list = tile_list; a.n_list = n_list;
   int grid = 0, P = 0, ols = 0;
-  // 64-wide nets with cached activations: tcgen05 kernel (update_umma.cu); without a cache the FP32 tiled-GEMM kernel
-  // 32-wide nets with cached activations: tcgen05 kernel (update_umma32.cu); without a cache the FP32 tile kernel
+  // 64-wide nets with cached activations: wgmma kernel (update_umma.cu); without a cache the FP32 tiled-GEMM kernel
+  // 32-wide nets with cached activations: wgmma kernel (update_umma32.cu); without a cache the FP32 tile kernel
 #ifdef B200RL_AB_TILE32
   int rc = (h1 == 32) ? update_tile_launch(MODE_FVP, obs_dim, act_dim, a, &grid, &P, &ols, st)
 #else

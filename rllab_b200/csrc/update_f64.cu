@@ -6,7 +6,8 @@
 // kernels evaluate the same three passes in float64 arithmetic on the float64 master parameters, which lets the whole
 // TRPO step be compared with the oracle at the reference's default settings.  They are deliberately simple -- one
 // thread per sample, weights in shared memory, weight gradients accumulated with shared-memory float64 atomics -- and
-// ~10x slower than the float32 kernels; B200's half-rate FP64 pipe makes that a usable verification mode.
+// ~10x slower than the float32 kernels; the half-rate FP64 pipe of the data-centre GPUs makes that a usable
+// verification mode.
 //
 // Same formulas and reference citations as update.cu / update_tile.cu.
 #include "update_common.cuh"

@@ -573,7 +573,7 @@ static int launch_gemm(const UpdArgs& a, int* grid_out, cudaStream_t st) {
 }
 
 // The shipped library reaches this FP32 formulation only for the Fisher-vector product without an activation cache (the
-// tcgen05 kernels serve b200rl_grad); its gradient instantiations are built for the A/B variant only
+// tensor-core kernels serve b200rl_grad); its gradient instantiations are built for the A/B variant only
 // (-DB200RL_AB_TILE32, README.md).
 namespace {   // per translation unit: update_tile.cu and update_gemm.cu each have their own
 #ifdef B200RL_AB_TILE32
@@ -588,7 +588,7 @@ struct FfmaGrad {
 template <class N>
 struct FfmaGrad<N, false> {
   static int run(const UpdArgs&, int*, cudaStream_t) {
-    set_error("the FP32 gradient kernels are not part of this build (the tcgen05 kernels serve b200rl_grad)");
+    set_error("the FP32 gradient kernels are not part of this build (the tensor-core kernels serve b200rl_grad)");
     return B200RL_EUNSUPPORTED;
   }
 };

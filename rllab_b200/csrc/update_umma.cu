@@ -1,36 +1,34 @@
-// Surrogate gradient and Fisher-vector product for 64-wide policies with the dense layer chain on the 5th-generation
-// tensor cores (tcgen05.mma.kind::tf32, accumulators and A operands in TMEM).  north_star: "tensor cores only for the dense
-// policy GEMM where hidden_dim >= 64".
+// Surrogate gradient and Fisher-vector product for 64-wide policies with the dense layer chain on the warpgroup tensor
+// cores (wgmma.mma_async .tf32: accumulators and A operands in registers, weight images in shared memory).
 //
 // The description below is the Fisher-vector pass (MODE_FVP).  The gradient pass (MODE_GRAD) runs the same pipeline with
-// the forward chain in place of the tangent chain: B  H1pre = X W0;  C  h1 = tanh(H1pre + b0) -> TMEM (and the activation
-// cache);  D  H2pre = H1 W1;  E  h2 = tanh(H2pre + b1), mean, log-likelihood, surrogate / KL terms, dmu, dlog_std, d2;
-// F, G, H as below.  Its forward is float32-grade, not bit-identical to the FFMA chain of the rollout (update_umma32.cu).
+// the forward chain in place of the tangent chain: B  H1pre = X W0;  C  h1 = tanh(H1pre + b0) -> A operand (and the
+// activation cache);  D  H2pre = H1 W1;  E  h2 = tanh(H2pre + b1), mean, log-likelihood, surrogate / KL terms, dmu,
+// dlog_std, d2;  F, G, H as below.  Its forward is float32-grade, not bit-identical to the FFMA chain of the rollout.
 //
-// Per 128-sample tile (one CTA of 256 threads per SM, persistent over tiles; samples = the 128 TMEM lanes):
-//   A   load X and the cached activations H1, H2 (written by b200rl_grad at the same theta); H1 / X -> TMEM A operands
-//       (tcgen05.st, hi + lo words) and -> feature-major fp32 rows in shared memory for the Gram phase
-//   B   MMA  T1pre = X V0          (K = 24)      and, queued behind it,  T2pre  = H1 V1   (independent of T1)
-//   C   epilogue: T1 = (T1pre + vb0)(1 - H1^2) -> TMEM A operand
+// Per 128-sample tile (one CTA of 256 threads = two warpgroups per SM, persistent over tiles; warpgroup w owns samples
+// 64 w .. 64 w + 63 of the tile, each thread two of them in the accumulator fragment layout of umma_common.cuh):
+//   A   load X and the cached activations H1 (written by b200rl_grad at the same theta) -> A-operand registers (hi + lo
+//       words) and -> feature-major fp32 rows in shared memory for the Gram phase
+//   B   MMA  T1pre = X V0          (K = obs_dim padded to 8)  and, in the same group,  T2pre = H1 V1
+//   C   epilogue: T1 = (T1pre + vb0)(1 - H1^2) -> A operand
 //   D   MMA  T2pre += T1 W1
-//   E   epilogue: T2 = (T2pre + vb1)(1 - H2^2); mu_dot = T2 Wout + H2 Vout + vbout (CUDA cores, N = A <= 3);
-//       dmu = M mu_dot; D2 = (dmu Wout^T)(1 - H2^2) -> TMEM A operand + shared-memory rows;
-//       dWout / dbout partial sums by a warp reduce-scatter of h2[j] dmu[k] (no H2 rows in shared memory)
-//   F   MMA  D1pre = D2 W1^T
+//   E   epilogue: T2 = (T2pre + vb1)(1 - H2^2); mu_dot = T2 Wout + H2 Vout + vbout (CUDA cores, N = A <= 3, the four
+//       threads of a row combine by shuffles); dmu = M mu_dot; D2 = (dmu Wout^T)(1 - H2^2) -> A operand + shared-memory rows
+//   F   MMA  D1pre = D2 W1^T, and behind it: dWout / dbout partial sums (warp reduce-scatter of h2[j] dmu[k])
 //   G   epilogue: D1 = D1pre (1 - H1^2) -> shared-memory rows
 //   H   Gram products on the CUDA cores (dW1 = H1^T D2, dW0 = X^T D1, db0, db1) exactly as update_gemm.cu
-// i.e. the five K = 64 / K = 24 GEMMs of the tangent-forward / backward chain (71 % of the multiply-adds of the pass) move
-// to the tensor cores; the sample-axis reductions stay on the FP32 pipe (their operands would need a second, transposed
-// set of hi/lo operand images in shared memory, which does not fit next to the weight images: DESIGN.md).
+// i.e. the K = 64 / K = obs_dim GEMMs of the tangent-forward / backward chain move to the tensor cores; the sample-axis
+// reductions stay on the FP32 pipe (their operands would need a second, transposed set of hi/lo operand images in shared
+// memory, which does not fit next to the weight images).
 //
-// Precision: float32-grade via the three-pass TF32 split  a b ~ a_hi b_hi + a_lo b_hi + a_hi b_lo  (hi = the word with its
-// 13 low mantissa bits cleared, exactly representable in TF32; lo = x - hi, exact in float32), accumulated in float32 in
-// TMEM, small terms first.  scripts/tf32_split_study.py: 4e-7 of the output scale, the same as the FFMA chains.
+// Precision: float32-grade via the three-pass TF32 split  a b ~ a_lo b_hi + a_hi b_lo + a_hi b_hi  (hi = the word with
+// its 13 low mantissa bits cleared, exactly representable in TF32; lo = x - hi, exact in float32), accumulated in float32,
+// small terms first.  scripts/tf32_split_study.py: 4e-7 of the output scale, the same as the FFMA chains.
 //
-// Operand formats (verified on a B200 with csrc/experimental/umma_modes_probe.cu): A from TMEM (lane = sample row, column
-// = k), B from shared memory in the canonical K-major no-swizzle layout (8 rows x 16 B core matrices): element (n, k) of a
-// [64 x K] image at (k%4)*4 + (n%8)*16 + (n/8)*128 + (k/4)*1024 bytes.  MN-major TF32 operands only exist in the
-// 128B_BASE32B swizzle, which is why every weight matrix gets its own K-major image (W1 both as [j][i] and [i][j]).
+// Operand formats: B = [64 x K] weight image in shared memory in the canonical K-major no-swizzle layout (8 rows x 16 B
+// core matrices): element (n, k) at (k%4)*4 + (n%8)*16 + (n/8)*128 + (k/4)*1024 bytes with k = u_kperm(input feature).
+// TF32 operands exist only K-major, which is why every weight matrix gets its own image (W1 both as [j][i] and [i][j]).
 //
 // Replaces f_Hx_plain of rllab/optimizers/conjugate_gradient_optimizer.py:22-55 (PerlmutterHvp) for hidden (64,64).
 #include "tile_phase_a.cuh"
@@ -39,15 +37,13 @@
 namespace b200rl {
 
 constexpr int U_THREADS = 256, U_TILE = 128, U_LD = U_TILE + 4, U_FLUSH = 8;
-constexpr int U_TMEM_COLS = 512;
-constexpr int U_cACC_A = 0, U_cACC_B = 64, U_cX_HI = 128, U_cX_LO = 152, U_cH1_HI = 192, U_cH1_LO = 256, U_cT_HI = 320,
-              U_cT_LO = 384;
-constexpr int U_KX = 24;   // obs columns of the X operand (O <= 20 padded with zeros to a multiple of 8)
+constexpr int U_KX = 24;   // obs columns of the X weight image (O <= 20 padded with zeros to a multiple of 8)
 
 template <class N, int MODE>
 struct UmmaSmem {
   static constexpr int O = N::O, H = 64, A = N::A;
-  static_assert(N::H1 == 64 && N::H2 == 64 && O <= U_KX, "tcgen05 Fisher-vector kernel: (64,64) nets, obs_dim <= 24");
+  static_assert(N::H1 == 64 && N::H2 == 64 && O <= U_KX, "tensor-core 64-wide kernel: (64,64) nets, obs_dim <= 24");
+  static constexpr int KSX = (O + 7) / 8;                                  // k-steps of the X GEMM
   static constexpr int IMG64 = 64 * 64 * 4, IMGX = 64 * U_KX * 4;            // bytes of one [64 x K] operand image
   // weight images (hi then lo): bW1T [j][i], bV1T [j][i] (FVP only), bW1 [i][j], bV0T [j][o] (GRAD: W0^T)
   static constexpr int o_bW1T = 0, o_bV1T = o_bW1T + 2 * IMG64, o_bW1 = o_bV1T + (MODE == MODE_FVP ? 2 * IMG64 : 0),
@@ -57,31 +53,30 @@ struct UmmaSmem {
   static constexpr int o_stage = o_small + n_small * 4;
   static constexpr int rX = 0, rH1 = rX + O, rD1 = rH1 + H, rD2 = rD1 + H, R = rD2 + H;
   static constexpr int o_red = ((o_stage + R * U_LD * 4 + 15) / 16) * 16;     // 3 x 32 doubles: loss / KL block reduction
-  static constexpr int o_bar = o_red + 3 * 32 * 8;
-  static constexpr size_t bytes = (size_t)o_bar + 64;
+  static constexpr size_t bytes = (size_t)o_red + 3 * 32 * 8;
   static_assert(bytes <= 232448, "does not fit the 227 KB of shared memory");
+  static_assert(8 * 200 * 4 <= H * U_LD * 4, "the D1 rows must hold the dWout / dbout combine scratch");
 };
 
-// element (n, k) of a K-major [64 x K] image, byte offset
-__device__ __forceinline__ int u_boff(int n, int k) { return (k & 3) * 4 + (n & 7) * 16 + (n >> 3) * 128 + (k >> 2) * 1024; }
+// element (n, k) of a K-major [64 x K] image, byte offset (k: input feature, stored at u_kperm(k))
+__device__ __forceinline__ int u_boff(int n, int k) {
+  const int kp = u_kperm(k);
+  return (kp & 3) * 4 + (n & 7) * 16 + (n >> 3) * 128 + (kp >> 2) * 1024;
+}
 
 template <class N, int MODE>
 __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) {
   using SM = UmmaSmem<N, MODE>;
-  constexpr int O = N::O, H = 64, A = N::A, P = N::P, LD = U_LD;
+  constexpr int O = N::O, H = 64, A = N::A, P = N::P, LD = U_LD, KSX = SM::KSX;
   extern __shared__ __align__(1024) unsigned char smem[];
   float* small = reinterpret_cast<float*>(smem + SM::o_small);
   float* sWout = small, *sVout = small + H * A, *svb0 = small + 2 * H * A, *svb1 = svb0 + H, *svbo = svb1 + H;
   float* stage = reinterpret_cast<float*>(smem + SM::o_stage);
   double* red_scratch = reinterpret_cast<double*>(smem + SM::o_red);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM::o_bar);           // [3] mbarriers, then the TMEM base holder
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(smem + SM::o_bar + 32);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int q = warp & 3, hf = warp >> 2;                                   // TMEM lane quadrant, unit half
-  const int srow = q * 32 + lane;                                           // sample row of this thread inside the tile
-  const int j0 = hf * 32;                                                   // first hidden unit of this thread
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, t4 = lane & 3;
+  const int row0 = (warp >> 2) * 64 + (warp & 3) * 16;                       // this warp's 16 rows of the tile
 
-  // ---- one-time setup: operand images of the weights, small parameters, barriers, TMEM
+  // ---- one-time setup: operand images of the weights, small parameters
   for (int e = tid; e < H * H; e += U_THREADS) {
     const int i = e / H, j = e % H;                                         // W1[i][j] (row-major in theta)
     const float w = a.params[N::oW1 + e];
@@ -116,22 +111,8 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
   if (tid < A) svbo[tid] = (MODE == MODE_FVP) ? (float)a.xvec[N::obo + tid] : a.params[N::obo + tid];
   double* out = a.partial + (size_t)blockIdx.x * P;
   for (int i = tid; i < P; i += U_THREADS) out[i] = 0.0;
-  if (tid == 0) {
-#pragma unroll
-    for (int b = 0; b < 3; ++b) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(u_smem_u32(&bars[b])));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(u_smem_u32(tmem_holder)),
-                 "r"(U_TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes of the images -> visible to UMMA
-  u_fence_before();
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes of the images -> visible to wgmma
   __syncthreads();
-  u_fence_after();
-  const uint32_t tbase = *tmem_holder;
-  const uint32_t tlane = tbase + ((uint32_t)(q * 32) << 16);                 // this warp's 32 lanes
 
   TileDist D;
   tile_dist_init<N, MODE>(D, a.params + N::ols, a);
@@ -139,17 +120,6 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
   const uint64_t dV1T_hi = u_desc(u_smem_u32(smem + SM::o_bV1T), 1024, 128), dV1T_lo = u_desc(u_smem_u32(smem + SM::o_bV1T + SM::IMG64), 1024, 128);
   const uint64_t dW1_hi = u_desc(u_smem_u32(smem + SM::o_bW1), 1024, 128), dW1_lo = u_desc(u_smem_u32(smem + SM::o_bW1 + SM::IMG64), 1024, 128);
   const uint64_t dV0T_hi = u_desc(u_smem_u32(smem + SM::o_bV0T), 1024, 128), dV0T_lo = u_desc(u_smem_u32(smem + SM::o_bV0T + SM::IMGX), 1024, 128);
-
-  // three-pass split GEMM over KS k-steps of 8: D (+)= A B, A hi/lo in TMEM, B hi/lo images in shared memory
-  auto split_gemm = [&](uint32_t d_col, uint32_t a_hi_col, uint32_t a_lo_col, uint64_t b_hi, uint64_t b_lo, int KS,
-                        bool accumulate) {
-    for (int ks = 0; ks < KS; ++ks) {
-      const uint64_t koff = (uint64_t)((ks * 2 * 1024) >> 4);               // 8 k = two 4-k core-matrix columns
-      u_mma_ts(tbase + d_col, tbase + a_lo_col + ks * 8, b_hi + koff, (accumulate || ks > 0) ? 1u : 0u);
-      u_mma_ts(tbase + d_col, tbase + a_hi_col + ks * 8, b_lo + koff, 1u);
-      u_mma_ts(tbase + d_col, tbase + a_hi_col + ks * 8, b_hi + koff, 1u);
-    }
-  };
 
   // ---- Gram ownership (as update_gemm.cu, 256 threads: one 4x4 tile of dW1 per thread)
   const int ti = tid / 16, tj = tid % 16;
@@ -165,15 +135,14 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
   float2 gS[OH + 1];
 #pragma unroll
   for (int k = 0; k <= OH; ++k) gS[k] = make_float2(0.f, 0.f);
-  float gWo[3] = {0.f, 0.f, 0.f};      // this lane's 3 entries of the warp's 32 x 3 block of dWout (reduce-scatter owner)
-  float gbo[A], gls[A];               // dbout, dlog_std (GRAD): lane 0 of the unit-half-0 warps
+  // dWout: the thread's 16 columns x 3 actions (flat c * 3 + k, c = 2 (column block) + column parity) are reduce-scattered
+  // over the eight row lanes of the warp; lane keeps flat indices wo_base .. wo_base + 5
+  float gWo[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  const int wo_base = ((lane >> 4) & 1) * 24 + ((lane >> 3) & 1) * 12 + ((lane >> 2) & 1) * 6;
+  float gbo[A], gls[A];               // dbout, dlog_std (GRAD): lane 0 of every warp
 #pragma unroll
   for (int k = 0; k < A; ++k) { gbo[k] = 0.f; gls[k] = 0.f; }
-  double s_loss = 0.0, s_kl = 0.0, m_kl = -1.0e300;   // GRAD: surrogate / KL terms, counted by the unit-half-0 thread
-  // flat index (j_local * 3 + k) of gWo[r]: the reduce-scatter keeps the lower / upper half by lane bits 4..0
-  const int wo_base = ((lane >> 4) & 1) * 48 + ((lane >> 3) & 1) * 24 + ((lane >> 2) & 1) * 12 + ((lane >> 1) & 1) * 6 +
-                      (lane & 1) * 3;
-  bool timed_out = false;
+  double s_loss = 0.0, s_kl = 0.0, m_kl = -1.0e300;   // GRAD: surrogate / KL terms, counted by the t4 == 0 thread of a row
 
   auto flush = [&]() {
     {
@@ -208,35 +177,37 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
     }
 #pragma unroll
     for (int k = 0; k <= OH; ++k) gS[k] = make_float2(0.f, 0.f);
-    // dWout / dbout: the four quadrant warps of a unit half hold partial sums of the same entries -> combine through the
-    // (idle) D1 rows in fixed warp order
-    float* scr = stage + SM::rD1 * LD;         // [8 warps][96 + 4]
+    // dWout / dbout / dlog_std: the eight warps hold partial sums of the same entries -> combine through the (idle) D1
+    // rows in fixed warp order.  scr[warp][200]: [col * 3 + k] dWout, [192 + k] dbout, [196 + k] dlog_std
+    float* scr = stage + SM::rD1 * LD;
 #pragma unroll
-    for (int r = 0; r < 3; ++r) scr[warp * 100 + wo_base + r] = gWo[r];
+    for (int r = 0; r < 6; ++r) {
+      const int f = wo_base + r, c = f / 3, k = f % 3;
+      if (k < A) scr[warp * 200 + (8 * (c >> 1) + 2 * t4 + (c & 1)) * 3 + k] = gWo[r];
+    }
     if (lane == 0)
 #pragma unroll
-      for (int k = 0; k < A; ++k) scr[warp * 100 + 96 + k] = gbo[k];
-    float* scl = scr + 8 * 100;                 // [4 quadrant warps of unit half 0][A]: dlog_std partial sums
-    if (MODE == MODE_GRAD && lane == 0 && hf == 0)
-#pragma unroll
-      for (int k = 0; k < A; ++k) scl[q * 4 + k] = gls[k];
-    __syncthreads();
-    if (tid < 2 * 96) {
-      const int h2 = tid / 96, f = tid % 96;   // unit half, flat (j_local, k) index
-      if (f % 3 < A) {
-        const float s4 = (scr[(h2 * 4 + 0) * 100 + f] + scr[(h2 * 4 + 1) * 100 + f]) +
-                         (scr[(h2 * 4 + 2) * 100 + f] + scr[(h2 * 4 + 3) * 100 + f]);
-        out[N::oWo + (h2 * 32 + f / 3) * A + (f % 3)] += (double)s4;
+      for (int k = 0; k < A; ++k) {
+        scr[warp * 200 + 192 + k] = gbo[k];
+        scr[warp * 200 + 196 + k] = gls[k];
       }
-    } else if (tid < 2 * 96 + A) {
-      const int k = tid - 2 * 96;
-      out[N::obo + k] += (double)((scr[0 * 100 + 96 + k] + scr[1 * 100 + 96 + k]) + (scr[2 * 100 + 96 + k] + scr[3 * 100 + 96 + k]));
-    } else if (MODE == MODE_GRAD && tid < 2 * 96 + 2 * A) {
-      const int k = tid - 2 * 96 - A;
-      out[N::ols + k] += (double)((scl[0 * 4 + k] + scl[1 * 4 + k]) + (scl[2 * 4 + k] + scl[3 * 4 + k]));
+    __syncthreads();
+    auto sum8 = [&](int idx) {
+      return ((scr[0 * 200 + idx] + scr[1 * 200 + idx]) + (scr[2 * 200 + idx] + scr[3 * 200 + idx])) +
+             ((scr[4 * 200 + idx] + scr[5 * 200 + idx]) + (scr[6 * 200 + idx] + scr[7 * 200 + idx]));
+    };
+    if (tid < H * A) {
+      const int col = tid / A, k = tid % A;
+      out[N::oWo + col * A + k] += (double)sum8(col * 3 + k);
+    } else if (tid < H * A + A) {
+      const int k = tid - H * A;
+      out[N::obo + k] += (double)sum8(192 + k);
+    } else if (MODE == MODE_GRAD && tid < H * A + 2 * A) {
+      const int k = tid - H * A - A;
+      out[N::ols + k] += (double)sum8(196 + k);
     }
 #pragma unroll
-    for (int r = 0; r < 3; ++r) gWo[r] = 0.f;
+    for (int r = 0; r < 6; ++r) gWo[r] = 0.f;
 #pragma unroll
     for (int k = 0; k < A; ++k) { gbo[k] = 0.f; gls[k] = 0.f; }
     __syncthreads();
@@ -244,271 +215,247 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
 
   const long long ntiles = n_tiles_of(a, U_TILE);
   int since_flush = 0;
-  uint32_t phase = 0;
-  for (long long ti_ = blockIdx.x; ti_ < ntiles; ti_ += gridDim.x, phase ^= 1u) {
+  for (long long ti_ = blockIdx.x; ti_ < ntiles; ti_ += gridDim.x) {
     const long long tile = tile_at(a, ti_);
-    const long long s = tile * U_TILE + srow;
-    const bool valid = sample_valid(a, s);
-    const long long sl = s < a.B ? s : a.B - 1;
-    // ================= A: loads; X / H1 -> TMEM A operands + feature-major rows
-    float h1[32], h2[32];
-    {
-      uint32_t hi[32], lo[32];
-      // observations: warps of unit half 0 own columns 0..15, half 1 columns 16..23 (zero padded)
+    long long sl[2];
+    bool valid[2], inrange[2];
+    int trow[2];                               // the thread's two rows inside the tile
 #pragma unroll
-      for (int c = 0; c < 16; ++c) {
-        const int o = hf * 16 + c;
+    for (int h = 0; h < 2; ++h) {
+      trow[h] = row0 + u_frag_row(2 * h, lane);
+      const long long s = tile * U_TILE + trow[h];
+      inrange[h] = s < a.B;
+      valid[h] = sample_valid(a, s);
+      sl[h] = inrange[h] ? s : a.B - 1;
+    }
+    // ================= A: loads; X / H1 -> A operands + feature-major rows
+    float accA[32], accB[32];
+    {
+      float xf[4 * KSX];
+#pragma unroll
+      for (int i = 0; i < 4 * KSX; ++i) {
+        const int o = u_frag_col(i, lane), h = (i >> 1) & 1;
         float x = 0.f;
         if (o < O) {
-          x = a.obs[(size_t)o * a.B + sl];
-          stage[(SM::rX + o) * LD + srow] = x;
+          x = a.obs[(size_t)o * a.B + sl[h]];
+          stage[(SM::rX + o) * LD + trow[h]] = x;
         }
-        const float xh = tf32_hi(x);
-        hi[c] = __float_as_uint(xh);
-        lo[c] = __float_as_uint(x - xh);
+        xf[i] = x;
       }
-      if (hf == 0) {
-        u_st16(tlane + U_cX_HI, hi, 0);
-        u_st16(tlane + U_cX_LO, lo, 0);
-      } else {
-        asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(tlane + U_cX_HI + 16),
-                     "r"(hi[0]), "r"(hi[1]), "r"(hi[2]), "r"(hi[3]), "r"(hi[4]), "r"(hi[5]), "r"(hi[6]), "r"(hi[7]) : "memory");
-        asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(tlane + U_cX_LO + 16),
-                     "r"(lo[0]), "r"(lo[1]), "r"(lo[2]), "r"(lo[3]), "r"(lo[4]), "r"(lo[5]), "r"(lo[6]), "r"(lo[7]) : "memory");
-      }
+      uint32_t xhi[4 * KSX], xlo[4 * KSX];
+      u_to_operand(xf, xhi, xlo);
+      // ================= B: T1pre = X V0 ; T2pre = H1 V1
       if constexpr (MODE == MODE_FVP) {
-        const float* hc = a.h_cache + sl;
+        float h1f[32];
+        const float* hc = a.h_cache;
 #pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          h1[c] = hc[(size_t)(j0 + c) * a.B];
-          h2[c] = hc[(size_t)(H + j0 + c) * a.B];
+        for (int i = 0; i < 32; ++i) {
+          const int c = u_frag_col(i, lane), h = (i >> 1) & 1;
+          h1f[i] = hc[(size_t)c * a.B + sl[h]];
+          stage[(SM::rH1 + c) * LD + trow[h]] = h1f[i];
         }
-#pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          stage[(SM::rH1 + j0 + c) * LD + srow] = h1[c];
-          const float hh = tf32_hi(h1[c]);
-          hi[c] = __float_as_uint(hh);
-          lo[c] = __float_as_uint(h1[c] - hh);
-        }
-        u_st32(tlane + U_cH1_HI + j0, hi);
-        u_st32(tlane + U_cH1_LO + j0, lo);
+        uint32_t hhi[32], hlo[32];
+        u_to_operand(h1f, hhi, hlo);
+        wg_fence();
+        wg_split_gemm(accA, xhi, xlo, dV0T_hi, dV0T_lo, 2048, KSX, false);      // X V0
+        wg_split_gemm(accB, hhi, hlo, dV1T_hi, dV1T_lo, 2048, 8, false);        // H1 V1
+        wg_commit();
+        wg_wait_all();
+      } else {
+        wg_fence();
+        wg_split_gemm(accA, xhi, xlo, dV0T_hi, dV0T_lo, 2048, KSX, false);      // GRAD: X W0
+        wg_commit();
       }
-      u_wait_st();
-    }
-    u_fence_before();
-    __syncthreads();
-    // ================= B: T1pre = X V0 ; T2pre = H1 V1
-    if (tid == 0) {
-      u_fence_after();
-      split_gemm(U_cACC_A, U_cX_HI, U_cX_LO, dV0T_hi, dV0T_lo, U_KX / 8, false);     // X V0  |  GRAD: X W0
-      u_commit(&bars[0]);
-      if constexpr (MODE == MODE_FVP) split_gemm(U_cACC_B, U_cH1_HI, U_cH1_LO, dV1T_hi, dV1T_lo, 8, false);
     }
     // GRAD: the remaining per-sample inputs, requested while the first GEMM runs
-    float act[A], om[A], adv_s = 0.f;
+    float act[2][A], om[2][A], adv_s[2] = {0.f, 0.f};
     if constexpr (MODE == MODE_GRAD) {
 #pragma unroll
-      for (int k = 0; k < A; ++k) {
-        act[k] = a.act[(size_t)k * a.B + sl];
-        om[k] = a.old_mean[(size_t)k * a.B + sl];
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int k = 0; k < A; ++k) {
+          act[h][k] = a.act[(size_t)k * a.B + sl[h]];
+          om[h][k] = a.old_mean[(size_t)k * a.B + sl[h]];
+        }
+        adv_s[h] = a.adv[sl[h]];
       }
-      adv_s = a.adv[sl];
+      wg_wait_all();
     }
-    // ================= C: T1 = (T1pre + vb0)(1 - H1^2) -> TMEM A operand
-    timed_out |= !u_wait(&bars[0], phase);
-    u_fence_after();
+    wg_fence_operand(accA);
+    wg_fence_operand(accB);
+    // ================= C: T1 = (T1pre + vb0)(1 - H1^2) -> A operand  |  GRAD: h1 = tanh(H1pre + b0)
     {
-      uint32_t r[32], lo[32];
-      u_ld32(tlane + U_cACC_A + j0, r);
+      float tf[32];
 #pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        float t1;                                 // the next A operand: t1 (FVP) | h1 (GRAD)
+      for (int i = 0; i < 32; ++i) {
+        const int c = u_frag_col(i, lane), h = (i >> 1) & 1;
         if constexpr (MODE == MODE_FVP) {
-          t1 = (__uint_as_float(r[c]) + svb0[j0 + c]) * (1.0f - h1[c] * h1[c]);
+          const float h1 = stage[(SM::rH1 + c) * LD + trow[h]];
+          tf[i] = (accA[i] + svb0[c]) * (1.0f - h1 * h1);
         } else {
-          t1 = tanh_f(__uint_as_float(r[c]) + svb0[j0 + c]);
-          h1[c] = t1;
-          stage[(SM::rH1 + j0 + c) * LD + srow] = t1;
-          if (a.h_cache != nullptr && s < a.B) a.h_cache[(size_t)(j0 + c) * a.B + s] = t1;
+          tf[i] = tanh_f(accA[i] + svb0[c]);
+          stage[(SM::rH1 + c) * LD + trow[h]] = tf[i];
+          if (a.h_cache != nullptr && inrange[h]) a.h_cache[(size_t)c * a.B + sl[h]] = tf[i];
         }
-        const float th = tf32_hi(t1);
-        r[c] = __float_as_uint(th);
-        lo[c] = __float_as_uint(t1 - th);
       }
-      u_st32(tlane + U_cT_HI + j0, r);
-      u_st32(tlane + U_cT_LO + j0, lo);
-      u_wait_st();
+      uint32_t thi[32], tlo[32];
+      u_to_operand(tf, thi, tlo);
+      // ================= D: T2pre += T1 W1  |  GRAD: H1 W1
+      wg_fence();
+      wg_split_gemm(accB, thi, tlo, dW1T_hi, dW1T_lo, 2048, 8, MODE == MODE_FVP);
+      wg_commit();
     }
-    u_fence_before();
-    __syncthreads();
-    // ================= D: T2pre += T1 W1
-    if (tid == 0) {
-      u_fence_after();
-      split_gemm(U_cACC_B, U_cT_HI, U_cT_LO, dW1T_hi, dW1T_lo, 8, MODE == MODE_FVP);   // += T1 W1  |  GRAD: H1 W1
-      u_commit(&bars[1]);
+    float h2f[32];
+    if constexpr (MODE == MODE_FVP) {               // cached h2, requested while the GEMM runs
+#pragma unroll
+      for (int i = 0; i < 32; ++i) h2f[i] = a.h_cache[(size_t)(H + u_frag_col(i, lane)) * a.B + sl[(i >> 1) & 1]];
     }
-    // ================= E: T2, mu_dot, dmu, D2 (+ dWout / dbout partial sums)
-    timed_out |= !u_wait(&bars[1], phase);
-    u_fence_after();
+    wg_wait_all();
+    wg_fence_operand(accB);
+    // ================= E: T2, mu_dot, dmu, D2  |  GRAD: h2, mean, surrogate / KL terms, dmu, dlog_std, D2
+    float dmu[2][A], dl[2][A];
     {
-      uint32_t r[32], lo[32];
-      u_ld32(tlane + U_cACC_B + j0, r);
-      float md[A];
+      float md[2][A];
 #pragma unroll
-      for (int k = 0; k < A; ++k) md[k] = 0.f;
+      for (int h = 0; h < 2; ++h)
 #pragma unroll
-      for (int c = 0; c < 32; ++c) {
+        for (int k = 0; k < A; ++k) md[h][k] = 0.f;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int c = u_frag_col(i, lane), h = (i >> 1) & 1;
         if constexpr (MODE == MODE_FVP) {
-          const float t2 = (__uint_as_float(r[c]) + svb1[j0 + c]) * (1.0f - h2[c] * h2[c]);
+          const float t2 = (accB[i] + svb1[c]) * (1.0f - h2f[i] * h2f[i]);
 #pragma unroll
-          for (int k = 0; k < A; ++k)
-            md[k] = fmaf(t2, sWout[(j0 + c) * A + k], fmaf(h2[c], sVout[(j0 + c) * A + k], md[k]));
+          for (int k = 0; k < A; ++k) md[h][k] = fmaf(t2, sWout[c * A + k], fmaf(h2f[i], sVout[c * A + k], md[h][k]));
         } else {
-          h2[c] = tanh_f(__uint_as_float(r[c]) + svb1[j0 + c]);
-          if (a.h_cache != nullptr && s < a.B) a.h_cache[(size_t)(H + j0 + c) * a.B + s] = h2[c];
+          h2f[i] = tanh_f(accB[i] + svb1[c]);
+          if (a.h_cache != nullptr && inrange[h]) a.h_cache[(size_t)(H + c) * a.B + sl[h]] = h2f[i];
 #pragma unroll
-          for (int k = 0; k < A; ++k) md[k] = fmaf(h2[c], sWout[(j0 + c) * A + k], md[k]);   // this half's part of the mean
+          for (int k = 0; k < A; ++k) md[h][k] = fmaf(h2f[i], sWout[c * A + k], md[h][k]);
         }
       }
-      // the two unit halves of a sample live in warps q and q + 4: exchange the partial sums through the idle D1 rows
-      float* xch = stage + SM::rD1 * LD;       // [2][128][4]
+      // the four threads of a row (t4 = 0..3) hold disjoint column sets: combine
 #pragma unroll
-      for (int k = 0; k < A; ++k) xch[(hf * U_TILE + srow) * 4 + k] = md[k];
-      __syncthreads();
-      float dmu[A], dl[A];
-      if constexpr (MODE == MODE_FVP) {
+      for (int h = 0; h < 2; ++h)
 #pragma unroll
         for (int k = 0; k < A; ++k) {
-          const float m = svbo[k] + (xch[srow * 4 + k] + xch[(U_TILE + srow) * 4 + k]);
-          dmu[k] = valid ? m * D.Mmu[k] : 0.f;
-          dl[k] = 0.f;
+          md[h][k] += __shfl_xor_sync(0xffffffffu, md[h][k], 1);
+          md[h][k] += __shfl_xor_sync(0xffffffffu, md[h][k], 2);
         }
-      } else {
-        // both unit halves of a sample evaluate the (cheap) distribution math; the half-0 thread counts the sample
-        float z[A], zsq = 0.f, zsq_old = 0.f, kl = 0.f;
 #pragma unroll
-        for (int k = 0; k < A; ++k) {
-          const float mu = svbo[k] + (xch[srow * 4 + k] + xch[(U_TILE + srow) * 4 + k]);
-          z[k] = (act[k] - mu) * D.inv_std[k];
-          zsq += z[k] * z[k];
-          const float zo = (act[k] - om[k]) * D.inv_std_old[k];
-          zsq_old += zo * zo;
-          const float dm = om[k] - mu;
-          kl += (dm * dm + D.var_old[k] - D.var_new[k]) / D.var_new2[k] + D.ls_new[k] - D.ls_old[k];
-        }
-        const float logp_new = -D.sum_ls_new - 0.5f * zsq - D.half_log2pi_A;
-        float w_s, term;
-        if (a.loss_kind == B200RL_LOSS_TRPO) {
-          const float logp_old = -D.sum_ls_old - 0.5f * zsq_old - D.half_log2pi_A;
-          w_s = expf(logp_new - logp_old) * adv_s;
-          term = -w_s;
+      for (int h = 0; h < 2; ++h) {
+        if constexpr (MODE == MODE_FVP) {
+#pragma unroll
+          for (int k = 0; k < A; ++k) {
+            dmu[h][k] = valid[h] ? (svbo[k] + md[h][k]) * D.Mmu[k] : 0.f;
+            dl[h][k] = 0.f;
+          }
         } else {
-          w_s = adv_s;
-          term = -logp_new * adv_s;
-        }
-        if (!valid) { w_s = 0.f; term = 0.f; }
-        if (hf == 0) {
-          s_loss += (double)term;
-          if (valid) { s_kl += (double)kl; m_kl = fmax(m_kl, (double)kl); }
-        }
+          float z[A], zsq = 0.f, zsq_old = 0.f, kl = 0.f;
 #pragma unroll
-        for (int k = 0; k < A; ++k) {
-          dmu[k] = -w_s * z[k] * D.inv_std[k];
-          dl[k] = -w_s * (z[k] * z[k] - 1.0f);
-        }
-      }
+          for (int k = 0; k < A; ++k) {
+            const float mu = svbo[k] + md[h][k];
+            z[k] = (act[h][k] - mu) * D.inv_std[k];
+            zsq += z[k] * z[k];
+            const float zo = (act[h][k] - om[h][k]) * D.inv_std_old[k];
+            zsq_old += zo * zo;
+            const float dm = om[h][k] - mu;
+            kl += (dm * dm + D.var_old[k] - D.var_new[k]) / D.var_new2[k] + D.ls_new[k] - D.ls_old[k];
+          }
+          const float logp_new = -D.sum_ls_new - 0.5f * zsq - D.half_log2pi_A;
+          float w_s, term;
+          if (a.loss_kind == B200RL_LOSS_TRPO) {
+            const float logp_old = -D.sum_ls_old - 0.5f * zsq_old - D.half_log2pi_A;
+            w_s = expf(logp_new - logp_old) * adv_s[h];
+            term = -w_s;
+          } else {
+            w_s = adv_s[h];
+            term = -logp_new * adv_s[h];
+          }
+          if (!valid[h]) { w_s = 0.f; term = 0.f; }
+          if (t4 == 0) {
+            s_loss += (double)term;
+            if (valid[h]) { s_kl += (double)kl; m_kl = fmax(m_kl, (double)kl); }
+          }
 #pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        float sacc = 0.f;
-#pragma unroll
-        for (int k = 0; k < A; ++k) sacc = fmaf(dmu[k], sWout[(j0 + c) * A + k], sacc);
-        const float d2 = sacc * (1.0f - h2[c] * h2[c]);
-        stage[(SM::rD2 + j0 + c) * LD + srow] = d2;
-        const float dh = tf32_hi(d2);
-        r[c] = __float_as_uint(dh);
-        lo[c] = __float_as_uint(d2 - dh);
-      }
-      u_st32(tlane + U_cT_HI + j0, r);
-      u_st32(tlane + U_cT_LO + j0, lo);
-      u_wait_st();
-      // warp reduce-scatter of h2[j] * dmu[k] ((j_local, k) flattened to 96 values) over the 32 samples of this warp:
-      // 48 + 24 + 12 + 6 + 3 shuffles, lane l ends with the sums of the flat indices wo_base .. wo_base + 2
-      float dm3[3];
-#pragma unroll
-      for (int k = 0; k < 3; ++k) dm3[k] = k < A ? dmu[k] : 0.f;
-      float pr[48];
-#pragma unroll
-      for (int i = 0; i < 48; ++i) {
-        const bool up = (lane >> 4) & 1;
-        const float plo = h2[i / 3] * dm3[i % 3], phi = h2[(48 + i) / 3] * dm3[(48 + i) % 3];
-        const float send = up ? plo : phi;
-        const float keep = up ? phi : plo;
-        pr[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-      }
-#pragma unroll
-      for (int i = 0; i < 24; ++i) {
-        const bool up = (lane >> 3) & 1;
-        const float send = up ? pr[i] : pr[24 + i];
-        const float keep = up ? pr[24 + i] : pr[i];
-        pr[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-      }
-#pragma unroll
-      for (int i = 0; i < 12; ++i) {
-        const bool up = (lane >> 2) & 1;
-        const float send = up ? pr[i] : pr[12 + i];
-        const float keep = up ? pr[12 + i] : pr[i];
-        pr[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-      }
-#pragma unroll
-      for (int i = 0; i < 6; ++i) {
-        const bool up = (lane >> 1) & 1;
-        const float send = up ? pr[i] : pr[6 + i];
-        const float keep = up ? pr[6 + i] : pr[i];
-        pr[i] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-      }
-#pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        const bool up = lane & 1;
-        const float send = up ? pr[i] : pr[3 + i];
-        const float keep = up ? pr[3 + i] : pr[i];
-        gWo[i] += keep + __shfl_xor_sync(0xffffffffu, send, 1);
-      }
-      if (hf == 0) {
-#pragma unroll
-        for (int k = 0; k < A; ++k) {
-          const float sdm = warp_sum(dmu[k]);
-          if (lane == 0) gbo[k] += sdm;
-          if constexpr (MODE == MODE_GRAD) {
-            const float sdl = warp_sum(dl[k]);
-            if (lane == 0) gls[k] += sdl;
+          for (int k = 0; k < A; ++k) {
+            dmu[h][k] = -w_s * z[k] * D.inv_std[k];
+            dl[h][k] = -w_s * (z[k] * z[k] - 1.0f);
           }
         }
       }
+      float d2f[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int c = u_frag_col(i, lane), h = (i >> 1) & 1;
+        float sacc = 0.f;
+#pragma unroll
+        for (int k = 0; k < A; ++k) sacc = fmaf(dmu[h][k], sWout[c * A + k], sacc);
+        d2f[i] = sacc * (1.0f - h2f[i] * h2f[i]);
+        stage[(SM::rD2 + c) * LD + trow[h]] = d2f[i];
+      }
+      uint32_t dhi[32], dlo[32];
+      u_to_operand(d2f, dhi, dlo);
+      // ================= F: D1pre = D2 W1^T
+      wg_fence();
+      wg_split_gemm(accA, dhi, dlo, dW1_hi, dW1_lo, 2048, 8, false);
+      wg_commit();
     }
-    u_fence_before();
-    __syncthreads();
-    // ================= F: D1pre = D2 W1^T
-    if (tid == 0) {
-      u_fence_after();
-      split_gemm(U_cACC_A, U_cT_HI, U_cT_LO, dW1_hi, dW1_lo, 8, false);
-      u_commit(&bars[2]);
+    // behind the GEMM: warp reduce-scatter of h2[j] * dmu[k] over the 16 rows of this warp (flat (c, k) index, 48 values:
+    // 24 + 12 + 6 shuffles); lane ends with the sums of the flat indices wo_base .. wo_base + 5
+    {
+      float dm3[2][3];
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int k = 0; k < 3; ++k) dm3[h][k] = k < A ? dmu[h][k] : 0.f;
+      auto val = [&](int f) {
+        const int c = f / 3, k = f % 3, i = 4 * (c >> 1) + (c & 1);
+        return h2f[i] * dm3[0][k] + h2f[i + 2] * dm3[1][k];
+      };
+      float pr[24];
+#pragma unroll
+      for (int i = 0; i < 24; ++i) {
+        const bool up = (lane >> 4) & 1;
+        const float plo = val(i), phi = val(24 + i);
+        pr[i] = (up ? phi : plo) + __shfl_xor_sync(0xffffffffu, up ? plo : phi, 16);
+      }
+#pragma unroll
+      for (int i = 0; i < 12; ++i) {
+        const bool up = (lane >> 3) & 1;
+        pr[i] = (up ? pr[12 + i] : pr[i]) + __shfl_xor_sync(0xffffffffu, up ? pr[i] : pr[12 + i], 8);
+      }
+#pragma unroll
+      for (int i = 0; i < 6; ++i) {
+        const bool up = (lane >> 2) & 1;
+        gWo[i] += (up ? pr[6 + i] : pr[i]) + __shfl_xor_sync(0xffffffffu, up ? pr[i] : pr[6 + i], 4);
+      }
+#pragma unroll
+      for (int k = 0; k < A; ++k) {
+        const float sdm = warp_sum(t4 == 0 ? dmu[0][k] + dmu[1][k] : 0.f);
+        if (lane == 0) gbo[k] += sdm;
+        if constexpr (MODE == MODE_GRAD) {
+          const float sdl = warp_sum(t4 == 0 ? dl[0][k] + dl[1][k] : 0.f);
+          if (lane == 0) gls[k] += sdl;
+        }
+      }
     }
     // ================= G: D1 = D1pre (1 - H1^2) -> rows
-    timed_out |= !u_wait(&bars[2], phase);
-    u_fence_after();
-    {
-      uint32_t r[32];
-      u_ld32(tlane + U_cACC_A + j0, r);
+    wg_wait_all();
+    wg_fence_operand(accA);
 #pragma unroll
-      for (int c = 0; c < 32; ++c) stage[(SM::rD1 + j0 + c) * LD + srow] = __uint_as_float(r[c]) * (1.0f - h1[c] * h1[c]);
+    for (int i = 0; i < 32; ++i) {
+      const int c = u_frag_col(i, lane), h = (i >> 1) & 1;
+      const float h1 = stage[(SM::rH1 + c) * LD + trow[h]];
+      stage[(SM::rD1 + c) * LD + trow[h]] = accA[i] * (1.0f - h1 * h1);
     }
-    u_fence_before();
     __syncthreads();
     // ================= H: Gram products over the tile (FP32 pipe)
     {
       // while the FP32 pipe works on this tile, pull the next tile's rows into L2 (its loads are otherwise fully exposed)
       const long long nti = ti_ + gridDim.x;
       if (nti < ntiles) {
+        const int q = warp & 3, hf = warp >> 2, j0 = hf * 32;
         const long long ns = tile_at(a, nti) * U_TILE + q * 32;      // one 128 B line per (row, warp): lane 0 fetches it
         if (lane == 0 && ns < a.B) {
           const float* hcn = a.h_cache + ns;
@@ -568,7 +515,6 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
     }
   }
   if (since_flush > 0) flush();
-  if (timed_out) out[tid % P] = __longlong_as_double(0x7FF8000000000000ll);   // an MMA never completed: poison the result
   if constexpr (MODE == MODE_GRAD) {
     __syncthreads();
     double v[2] = {s_loss, s_kl};
@@ -577,16 +523,13 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
     block_reduce_store<2, false>(v, red_scratch, sc);
     block_reduce_store<1, true>(mx, red_scratch, sc + 2);
   }
-  u_fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tbase), "r"(U_TMEM_COLS));
 }
 
 template <class N, int MODE>
 static int launch_umma(const UpdArgs& a, int* grid_out, cudaStream_t st) {
   using SM = UmmaSmem<N, MODE>;
   B200RL_SET_MAX_SMEM((update_umma64_kernel<N, MODE>), SM::bytes);
-  long long grid = num_sms();                      // one CTA per SM (512 TMEM columns, 220 KB of shared memory)
+  long long grid = num_sms();                      // one CTA per SM (up to 220 KB of shared memory)
   const long long ntiles = host_n_tiles(a, U_TILE);
   if (grid > ntiles) grid = ntiles;
   if (grid < 1) grid = 1;

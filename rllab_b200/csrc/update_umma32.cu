@@ -1,30 +1,31 @@
-// Surrogate gradient and Fisher-vector product for 32-wide policies with the dense layer chain on the 5th-generation
-// tensor cores (tcgen05.mma.kind::tf32, accumulators and A operands in TMEM) -- the 32-wide sibling of update_umma.cu.
+// Surrogate gradient and Fisher-vector product for 32-wide policies with the dense layer chain on the warpgroup tensor
+// cores (wgmma.mma_async .tf32, accumulators and A operands in registers) -- the 32-wide sibling of update_umma.cu.
 //
-// One CTA of 128 threads per 128-sample tile, two CTAs resident per SM (persistent over tiles), thread <-> sample <-> TMEM
-// lane.  The CUDA cores only do what is elementwise per sample (bias, tanh, the distribution math, (1 - h^2) factors, the
-// hi/lo operand split) and the sample-axis Gram products (tile_gram.cuh); every dense layer is a 128 x 32 x K tensor-core
-// GEMM whose A operand the previous epilogue wrote to TMEM with tcgen05.st:
+// One CTA of 128 threads (one warpgroup) per 128-sample tile, several CTAs resident per SM (persistent over tiles).  The
+// warpgroup covers the tile as two 64-row MMA blocks; each thread holds four samples of it in the accumulator fragment
+// layout of umma_common.cuh.  The CUDA cores only do what is elementwise per sample (bias, tanh, the distribution math,
+// (1 - h^2) factors, the hi/lo operand split) and the sample-axis Gram products (tile_gram.cuh); every dense layer is a
+// 128 x 32 x K tensor-core GEMM whose A operand the previous epilogue left in registers:
 //
-//   GRAD   A  x -> TMEM                         MMA  H1pre = X W0                  (K = obs_dim padded to 8)
-//          E1 h1 = tanh(H1pre + b0) -> TMEM     MMA  H2pre = H1 W1
+//   GRAD   A  x -> A operand                    MMA  H1pre = X W0                  (K = obs_dim padded to 8)
+//          E1 h1 = tanh(H1pre + b0)             MMA  H2pre = H1 W1
 //          E2 h2 = tanh(H2pre + b1); mean, log-likelihood, surrogate / KL terms, dmu, dlog_std;
-//             d2 = (dmu Wout^T)(1 - h2^2) -> TMEM                                  MMA  D1pre = D2 W1^T
+//             d2 = (dmu Wout^T)(1 - h2^2)                                          MMA  D1pre = D2 W1^T
 //          E3 d1 = D1pre (1 - h1^2)             Gram products (FP32 pipe)
-//   FVP    A  x, cached h1 / h2; X, H1 -> TMEM  MMA  T1pre = X V0 ; T2pre = H1 V1
-//          C  t1 = (T1pre + vb0)(1 - h1^2) -> TMEM                                 MMA  T2pre += T1 W1
-//          E  t2 = (T2pre + vb1)(1 - h2^2); mu_dot; dmu = M mu_dot; d2 -> TMEM     MMA  D1pre = D2 W1^T
+//   FVP    A  x, cached h1 / h2                 MMA  T1pre = X V0 ; T2pre = H1 V1
+//          C  t1 = (T1pre + vb0)(1 - h1^2)                                         MMA  T2pre += T1 W1
+//          E  t2 = (T2pre + vb1)(1 - h2^2); mu_dot; dmu = M mu_dot; d2             MMA  D1pre = D2 W1^T
 //          G  d1 = D1pre (1 - h1^2)             Gram products
 //
-// Against update_tile.cu (the same passes with FFMA2 chains, 134 warp-instructions per sample on cfg2) this removes the
-// 2 200 FMA + 550 weight LDS per sample of the layer chain from the issue slots and the LSU.  Precision: the three-pass
-// TF32 split a b ~ a_lo b_hi + a_hi b_lo + a_hi b_hi with float32 accumulation in TMEM (update_umma.cu; 4e-7 of the output
-// scale).  The tensor-core forward is NOT bit-identical to the FFMA chain of the rollout / loss kernels: the (loss, KL)
-// triple a gradient pass emits at theta_old is -mean(adv) and 0 to ~1e-7 instead of exactly; b200rl_loss_kl keeps the
-// exact property.
+// Against update_tile.cu (the same passes with FFMA chains) this removes the 2 200 FMA + 550 weight LDS per sample of the
+// layer chain from the issue slots and the LSU.  Precision: the three-pass TF32 split a b ~ a_lo b_hi + a_hi b_lo + a_hi
+// b_hi with float32 accumulation (update_umma.cu; 4e-7 of the output scale).  The tensor-core forward is NOT
+// bit-identical to the FFMA chain of the rollout / loss kernels: the (loss, KL) triple a gradient pass emits at theta_old
+// is -mean(adv) and 0 to ~1e-7 instead of exactly; the forward-only mode (MODE_LOSS) runs the gradient pass's forward
+// instruction for instruction, so the two agree bit for bit at equal theta.
 //
-// Operand formats as update_umma.cu: A from TMEM (lane = sample, column = k); B = [32 x K] weight image in shared memory,
-// K-major no-swizzle: element (n, k) at (k%4)*4 + (n%8)*16 + (n/8)*128 + (k/4)*512 bytes (LBO 512, SBO 128).
+// Operand formats as update_umma.cu: B = [32 x K] weight image in shared memory, K-major no-swizzle: element (n, k) at
+// (k%4)*4 + (n%8)*16 + (n/8)*128 + (k/4)*512 bytes, k = u_kperm(input feature) (LBO 512, SBO 128).
 //
 // Replaces f_grad / f_Hx_plain of rllab/optimizers/conjugate_gradient_optimizer.py:184-215,22-55 and the gradient half of
 // f_opt in rllab/optimizers/first_order_optimizer.py:62-76 for hidden (32,32).
@@ -35,22 +36,17 @@ namespace b200rl {
 
 constexpr int V_THREADS = 128, V_TILE = 128, V_LD = V_TILE + 4;
 #ifndef B200RL_V_PACKED_GRAM
-#define B200RL_V_PACKED_GRAM 1          // dW1 Gram with packed FFMA2 (A/B on a B200: see DESIGN.md)
+#define B200RL_V_PACKED_GRAM 1          // dW1 Gram with even / odd packed partial sums (tile_gram.cuh)
 #endif
 #ifndef B200RL_V_MAXB
-#define B200RL_V_MAXB 3                 // resident CTAs per SM where shared memory / TMEM / registers allow
-#endif
+#define B200RL_V_MAXB 2                 // resident CTAs per SM of the gradient / Fisher passes: at three (168 registers)
+#endif                                  // the gradient pass spills
 
 template <class N, int MODE>
 struct Umma32 {
   static constexpr int O = N::O, H = 32, A = N::A;
-  static_assert(N::H1 == 32 && N::H2 == 32 && O <= 24, "tcgen05 32-wide kernel: (32,32) nets, obs_dim <= 24");
+  static_assert(N::H1 == 32 && N::H2 == 32 && O <= 24, "tensor-core 32-wide kernel: (32,32) nets, obs_dim <= 24");
   static constexpr int KX = ((O + 7) / 8) * 8;                 // obs columns of the X operand, zero padded
-  // TMEM columns (float32 each): accumulators (the gradient pass uses them strictly one after the other: one slot), X
-  // hi/lo, one A-operand slot (H1, then T1 / D2) hi/lo
-  static constexpr int cACC_A = 0, cACC_B = (MODE == MODE_FVP) ? 32 : 0, cX_HI = cACC_B + 32, cX_LO = cX_HI + KX,
-                       cOP_HI = cX_LO + KX, cOP_LO = cOP_HI + 32, cEND = cOP_LO + 32;
-  static constexpr int TMEM_COLS = cEND <= 128 ? 128 : 256;
   static constexpr int IMG = 32 * 32 * 4, IMGX = 32 * KX * 4;   // bytes of one [32 x K] operand image
   // weight images (hi then lo).  GRAD: W0^T [j][o], W1^T [j][i], W1 [i][j].  FVP: V0^T, V1^T, W1^T, W1.
   // LOSS (forward only): W0^T, W1^T.
@@ -65,43 +61,34 @@ struct Umma32 {
   static constexpr int rX = 0, rH1 = rX + O, rH2 = rH1 + H, rD1 = rH2, rD2 = rH2 + H, rDM = rD2 + H, rDL = rDM + A,
                        R = (MODE == MODE_LOSS) ? 0 : rDL + A;
   static constexpr int o_red = ((o_stage + R * V_LD * 4 + 15) / 16) * 16;   // 3 x 32 doubles of reduction scratch
-  static constexpr int o_bar = o_red + 3 * 32 * 8;
-  // the forward-only pass needs 11 KB; it asks for enough that a fifth CTA cannot become resident on an SM (registers would
-  // allow it): every resident CTA must be able to allocate its 128 TMEM columns, and there are 512
-  static constexpr size_t need = (size_t)o_bar + 64, floor4 = (228 * 1024) / 5 + 1;
-  static constexpr size_t bytes = (MODE == MODE_LOSS && need < floor4) ? floor4 : need;
+  static constexpr size_t bytes = (size_t)o_red + 3 * 32 * 8;
   static_assert(MODE == MODE_LOSS || 2 * 64 * 16 * 8 <= R * V_LD * 4, "stage region must hold the K-half combine scratch");
   static_assert(bytes <= 232448, "does not fit the 227 KB of shared memory");
-  // resident CTAs per SM: shared memory (228 KB, 1 KB reserved per CTA), TMEM (512 columns), registers (64 K / 128 threads)
-  static constexpr int by_smem = (int)((228 * 1024) / (bytes + 1024)), by_tmem = 512 / TMEM_COLS;
-  static constexpr int cap = (MODE == MODE_LOSS) ? 4 : B200RL_V_MAXB, by_res = by_smem < by_tmem ? by_smem : by_tmem;
-  static constexpr int MINB = by_res < cap ? (by_res < 1 ? 1 : by_res) : cap;
+  // resident CTAs per SM: shared memory (228 KB, 1 KB reserved per CTA), registers (64 K / 128 threads)
+  static constexpr int by_smem = (int)((228 * 1024) / (bytes + 1024));
+  static constexpr int cap = (MODE == MODE_LOSS) ? 3 : B200RL_V_MAXB;
+  static constexpr int MINB = by_smem < cap ? (by_smem < 1 ? 1 : by_smem) : cap;
 };
 
-// element (n, k) of a K-major [32 x K] image, byte offset
-__device__ __forceinline__ int v_boff(int n, int k) { return (k & 3) * 4 + (n & 7) * 16 + (n >> 3) * 128 + (k >> 2) * 512; }
-
-__device__ __forceinline__ void v_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
+// element (n, k) of a K-major [32 x K] image, byte offset (k: input feature, stored at u_kperm(k))
+__device__ __forceinline__ int v_boff(int n, int k) {
+  const int kp = u_kperm(k);
+  return (kp & 3) * 4 + (n & 7) * 16 + (n >> 3) * 128 + (kp >> 2) * 512;
 }
 
 template <class N, int MODE>
 __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umma32_kernel(UpdArgs a) {
   using SM = Umma32<N, MODE>;
-  constexpr int O = N::O, H = 32, A = N::A, P = N::P, LD = V_LD, KX = SM::KX;
-  constexpr uint32_t IDESC = u_idesc(128, 32);
+  constexpr int O = N::O, H = 32, A = N::A, P = N::P, LD = V_LD, KX = SM::KX, KSX = KX / 8;
   extern __shared__ __align__(1024) unsigned char smem[];
   float* small = reinterpret_cast<float*>(smem + SM::o_small);
   float* sb0 = small, *sb1 = small + H, *sWout = small + 2 * H, *sVout = sWout + H * A;   // sVout: FVP only
   float* sbo = (MODE == MODE_FVP) ? sVout + H * A : sWout + H * A;
   float* stage = reinterpret_cast<float*>(smem + SM::o_stage);
   double* red_scratch = reinterpret_cast<double*>(smem + SM::o_red);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM::o_bar);           // [3] mbarriers, then the TMEM base holder
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(smem + SM::o_bar + 32);
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, t4 = lane & 3;
 
-  // ---- one-time setup: operand images of the weights, small parameters, barriers, TMEM
+  // ---- one-time setup: operand images of the weights, small parameters
   // MODE_GRAD: the chain multiplies by theta (params); MODE_FVP: first layers by the tangent x (xvec), W1 by theta
   for (int e = tid; e < H * H; e += V_THREADS) {
     const int i = e / H, j = e % H;                                         // W1[i][j] (row-major in theta)
@@ -137,22 +124,8 @@ __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umm
     sb1[e] = (MODE == MODE_FVP) ? (float)a.xvec[N::ob1 + e] : a.params[N::ob1 + e];
   }
   if (tid < A) sbo[tid] = (MODE == MODE_FVP) ? (float)a.xvec[N::obo + tid] : a.params[N::obo + tid];
-  if (tid == 0) {
-#pragma unroll
-    for (int b = 0; b < 3; ++b) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(u_smem_u32(&bars[b])));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(u_smem_u32(tmem_holder)),
-                 "r"(SM::TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes of the images -> visible to UMMA
-  u_fence_before();
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes of the images -> visible to wgmma
   __syncthreads();
-  u_fence_after();
-  const uint32_t tbase = *tmem_holder;
-  const uint32_t tlane = tbase + ((uint32_t)(warp * 32) << 16);               // this warp's 32 lanes
 
   TileDist D;
   tile_dist_init<N, MODE>(D, a.params + N::ols, a);
@@ -162,243 +135,257 @@ __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umm
   const uint64_t dW1_hi = u_desc(u_smem_u32(smem + SM::o_bW1), 512, 128), dW1_lo = u_desc(u_smem_u32(smem + SM::o_bW1 + SM::IMG), 512, 128);
   const uint64_t dV1T_hi = u_desc(u_smem_u32(smem + SM::o_bV1T), 512, 128), dV1T_lo = u_desc(u_smem_u32(smem + SM::o_bV1T + SM::IMG), 512, 128);
 
-  // three-pass split GEMM over KS k-steps of 8: D (+)= A B, A hi/lo in TMEM, B hi/lo images in shared memory
-  auto split_gemm = [&](uint32_t d_col, uint32_t a_hi_col, uint32_t a_lo_col, uint64_t b_hi, uint64_t b_lo, int KS,
-                        bool accumulate) {
-    for (int ks = 0; ks < KS; ++ks) {
-      const uint64_t koff = (uint64_t)((ks * 2 * 512) >> 4);                // 8 k = two 4-k core-matrix columns
-      u_mma_ts(tbase + d_col, tbase + a_lo_col + ks * 8, b_hi + koff, (accumulate || ks > 0) ? 1u : 0u, IDESC);
-      u_mma_ts(tbase + d_col, tbase + a_hi_col + ks * 8, b_lo + koff, 1u, IDESC);
-      u_mma_ts(tbase + d_col, tbase + a_hi_col + ks * 8, b_hi + koff, 1u, IDESC);
-    }
-  };
-  // 32 values of this sample -> the A-operand slot (hi + lo words)
-  auto put_operand = [&](const float (&v)[32]) {
-    uint32_t hi[32], lo[32];
+  // split GEMM of both 64-row blocks: acc[mb] (+)= f[mb] B, f[mb]: accumulator-ordered A values of KS k-steps
+  auto gemm2 = [&](float (&acc)[2][16], auto& f, uint64_t b_hi, uint64_t b_lo, int KS, bool accumulate) {
+    constexpr int NV = sizeof(f[0]) / sizeof(float);
 #pragma unroll
-    for (int c = 0; c < 32; ++c) {
-      const float vh = tf32_hi(v[c]);
-      hi[c] = __float_as_uint(vh);
-      lo[c] = __float_as_uint(v[c] - vh);
+    for (int mb = 0; mb < 2; ++mb) {
+      uint32_t hi[NV], lo[NV];
+      u_to_operand(f[mb], hi, lo);
+      wg_split_gemm(acc[mb], hi, lo, b_hi, b_lo, 1024, KS, accumulate);
     }
-    u_st32(tlane + SM::cOP_HI, hi);
-    u_st32(tlane + SM::cOP_LO, lo);
-    u_wait_st();
   };
 
   TileGram<N, SM::rX, SM::rH1, SM::rH2, SM::rD1, SM::rD2, SM::rDM, LD, B200RL_V_PACKED_GRAM != 0> gram;
   if constexpr (MODE != MODE_LOSS) gram.init();
   double s_loss = 0.0, s_kl = 0.0, m_kl = -1.0e300;
-  bool timed_out = false;
-
-  float* colX = stage + SM::rX * LD + tid;
-  float* colH1 = stage + SM::rH1 * LD + tid;
-  float* colH2 = stage + SM::rH2 * LD + tid;
-  float* colD1 = stage + SM::rD1 * LD + tid;
-  float* colD2 = stage + SM::rD2 * LD + tid;
-  float* colDM = stage + SM::rDM * LD + tid;
-  float* colDL = stage + SM::rDL * LD + tid;
 
   const long long ntiles = n_tiles_of(a, V_TILE);
-  uint32_t phase = 0;
-  for (long long ti_ = blockIdx.x; ti_ < ntiles; ti_ += gridDim.x, phase ^= 1u) {
-    const long long s = tile_at(a, ti_) * V_TILE + tid;
-    const bool inrange = s < a.B;
-    const bool valid = sample_valid(a, s);
-    const long long sl = inrange ? s : a.B - 1;
-    // ================= A: observations -> TMEM X operand + stage rows; FVP: cached activations, H1 -> operand slot
-    float h1[H], h2[H];
+  for (long long ti_ = blockIdx.x; ti_ < ntiles; ti_ += gridDim.x) {
+    const long long tile = tile_at(a, ti_);
+    // the thread's four samples: rows trow[mb][h] of the tile
+    int trow[2][2];
+    long long sl[2][2];
+    bool inrange[2][2], valid[2][2];
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        trow[mb][h] = mb * 64 + warp * 16 + u_frag_row(2 * h, lane);
+        const long long s = tile * V_TILE + trow[mb][h];
+        inrange[mb][h] = s < a.B;
+        valid[mb][h] = sample_valid(a, s);
+        sl[mb][h] = inrange[mb][h] ? s : a.B - 1;
+      }
+    float accA[2][16], accB[2][16];
+    // ================= A: observations -> X operand + stage rows; FVP: cached activations, H1 -> operand
     {
-      uint32_t hi[KX], lo[KX];
+      float xf[2][4 * KSX];
 #pragma unroll
-      for (int o = 0; o < KX; ++o) {
-        float x = 0.f;
-        if (o < O) {
-          x = a.obs[(size_t)o * a.B + sl];
-          if constexpr (MODE != MODE_LOSS) colX[o * LD] = x;
+      for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int i = 0; i < 4 * KSX; ++i) {
+          const int o = u_frag_col(i, lane), h = (i >> 1) & 1;
+          float x = 0.f;
+          if (o < O) {
+            x = a.obs[(size_t)o * a.B + sl[mb][h]];
+            if constexpr (MODE != MODE_LOSS) stage[(SM::rX + o) * LD + trow[mb][h]] = x;
+          }
+          xf[mb][i] = x;
         }
-        const float xh = tf32_hi(x);
-        hi[o] = __float_as_uint(xh);
-        lo[o] = __float_as_uint(x - xh);
-      }
+      if constexpr (MODE == MODE_FVP) {
+        float h1f[2][16];
 #pragma unroll
-      for (int o = 0; o < KX; o += 8) {
-        v_st8(tlane + SM::cX_HI + o, hi + o);
-        v_st8(tlane + SM::cX_LO + o, lo + o);
+        for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            const int c = u_frag_col(i, lane), h = (i >> 1) & 1;
+            h1f[mb][i] = a.h_cache[(size_t)c * a.B + sl[mb][h]];
+            stage[(SM::rH1 + c) * LD + trow[mb][h]] = h1f[mb][i];
+          }
+        wg_fence();
+        gemm2(accA, xf, dXT_hi, dXT_lo, KSX, false);                  // X V0
+        gemm2(accB, h1f, dV1T_hi, dV1T_lo, 4, false);                 // H1 V1
+        wg_commit();
+      } else {
+        wg_fence();
+        gemm2(accA, xf, dXT_hi, dXT_lo, KSX, false);                  // X W0
+        wg_commit();
       }
     }
-    if constexpr (MODE == MODE_FVP) {
-      const float* hc = a.h_cache + sl;
-#pragma unroll
-      for (int c = 0; c < H; ++c) {
-        h1[c] = hc[(size_t)c * a.B];
-        h2[c] = hc[(size_t)(H + c) * a.B];
-      }
-#pragma unroll
-      for (int c = 0; c < H; ++c) colH1[c * LD] = h1[c];
-      put_operand(h1);
-    } else {
-      u_wait_st();
-    }
-    u_fence_before();
-    __syncthreads();
-    if (tid == 0) {
-      u_fence_after();
-      split_gemm(SM::cACC_A, SM::cX_HI, SM::cX_LO, dXT_hi, dXT_lo, KX / 8, false);              // X W0  |  X V0
-      if constexpr (MODE == MODE_FVP)
-        split_gemm(SM::cACC_B, SM::cOP_HI, SM::cOP_LO, dV1T_hi, dV1T_lo, 4, false);            // H1 V1
-      u_commit(&bars[0]);
-    }
-    // GRAD / LOSS: the remaining per-sample inputs, requested while the first GEMM runs (prefetching them and the
-    // observations one tile ahead in registers was measured: no gain, 2.05 -> 2.07 ms)
-    float act[A], om[A], adv_s = 0.f;
+    // GRAD / LOSS: the remaining per-sample inputs, requested while the first GEMM runs
+    float act[2][2][A], om[2][2][A], adv_s[2][2];
     if constexpr (MODE != MODE_FVP) {
 #pragma unroll
-      for (int k = 0; k < A; ++k) {
-        act[k] = a.act[(size_t)k * a.B + sl];
-        om[k] = a.old_mean[(size_t)k * a.B + sl];
-      }
-      adv_s = a.adv[sl];
-    }
-    timed_out |= !u_wait(&bars[0], phase);
-    u_fence_after();
-    // ================= E1 / C: first epilogue
-    {
-      uint32_t r[32];
-      u_ld32(tlane + SM::cACC_A, r);
-      float v[32];
-      if constexpr (MODE != MODE_FVP) {
+      for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-        for (int c = 0; c < H; ++c) {
-          h1[c] = tanh_f(__uint_as_float(r[c]) + sb0[c]);
-          if constexpr (MODE == MODE_GRAD) colH1[c * LD] = h1[c];
-          v[c] = h1[c];
-        }
-        if (MODE == MODE_GRAD && a.h_cache != nullptr && inrange) {
-#pragma unroll
-          for (int c = 0; c < H; ++c) a.h_cache[(size_t)c * a.B + sl] = h1[c];
-        }
-      } else {
-#pragma unroll
-        for (int c = 0; c < H; ++c) v[c] = (__uint_as_float(r[c]) + sb0[c]) * (1.0f - h1[c] * h1[c]);   // t1
-      }
-      put_operand(v);
-    }
-    u_fence_before();
-    __syncthreads();
-    if (tid == 0) {
-      u_fence_after();
-      split_gemm(SM::cACC_B, SM::cOP_HI, SM::cOP_LO, dW1T_hi, dW1T_lo, 4, MODE == MODE_FVP);   // H1 W1  |  += T1 W1
-      u_commit(&bars[1]);
-    }
-    timed_out |= !u_wait(&bars[1], phase);
-    u_fence_after();
-    // ================= E2 / E: second epilogue -> dmu, d2
-    {
-      uint32_t r[32];
-      u_ld32(tlane + SM::cACC_B, r);
-      float dmu[A];
-      if constexpr (MODE != MODE_FVP) {
-#pragma unroll
-        for (int c = 0; c < H; ++c) {
-          h2[c] = tanh_f(__uint_as_float(r[c]) + sb1[c]);
-          if constexpr (MODE == MODE_GRAD) colH2[c * LD] = h2[c];
-        }
-        if (MODE == MODE_GRAD && a.h_cache != nullptr && inrange) {
-#pragma unroll
-          for (int c = 0; c < H; ++c) a.h_cache[(size_t)(H + c) * a.B + sl] = h2[c];
-        }
-        float z[A], zsq = 0.f, zsq_old = 0.f, kl = 0.f;
-#pragma unroll
-        for (int k = 0; k < A; ++k) {
-          float s0 = sbo[k], s1 = 0.f;                        // canonical even / odd order of mlp.cuh
-#pragma unroll
-          for (int j = 0; j < H; j += 2) {
-            s0 = fmaf(h2[j], sWout[j * A + k], s0);
-            s1 = fmaf(h2[j + 1], sWout[(j + 1) * A + k], s1);
-          }
-          const float mu = s0 + s1;
-          z[k] = (act[k] - mu) * D.inv_std[k];
-          zsq += z[k] * z[k];
-          const float zo = (act[k] - om[k]) * D.inv_std_old[k];
-          zsq_old += zo * zo;
-          const float dm = om[k] - mu;
-          kl += (dm * dm + D.var_old[k] - D.var_new[k]) / D.var_new2[k] + D.ls_new[k] - D.ls_old[k];
-        }
-        const float logp_new = -D.sum_ls_new - 0.5f * zsq - D.half_log2pi_A;
-        float w_s, term;
-        if (a.loss_kind == B200RL_LOSS_TRPO) {
-          const float logp_old = -D.sum_ls_old - 0.5f * zsq_old - D.half_log2pi_A;
-          w_s = expf(logp_new - logp_old) * adv_s;
-          term = -w_s;
-        } else {
-          w_s = adv_s;
-          term = -logp_new * adv_s;
-        }
-        if (!valid) { w_s = 0.f; term = 0.f; }
-        s_loss += (double)term;
-        if (valid) { s_kl += (double)kl; m_kl = fmax(m_kl, (double)kl); }
-        if constexpr (MODE == MODE_GRAD) {
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
           for (int k = 0; k < A; ++k) {
-            dmu[k] = -w_s * z[k] * D.inv_std[k];
-            colDM[k * LD] = dmu[k];
-            colDL[k * LD] = -w_s * (z[k] * z[k] - 1.0f);
+            act[mb][h][k] = a.act[(size_t)k * a.B + sl[mb][h]];
+            om[mb][h][k] = a.old_mean[(size_t)k * a.B + sl[mb][h]];
+          }
+          adv_s[mb][h] = a.adv[sl[mb][h]];
+        }
+    }
+    wg_wait_all();
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) {
+      wg_fence_operand(accA[mb]);
+      wg_fence_operand(accB[mb]);
+    }
+    // ================= E1 / C: first epilogue -> operand of the second GEMM
+    {
+      float v[2][16];
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const int c = u_frag_col(i, lane), h = (i >> 1) & 1;
+          if constexpr (MODE != MODE_FVP) {
+            v[mb][i] = tanh_f(accA[mb][i] + sb0[c]);
+            if constexpr (MODE == MODE_GRAD) {
+              stage[(SM::rH1 + c) * LD + trow[mb][h]] = v[mb][i];
+              if (a.h_cache != nullptr && inrange[mb][h]) a.h_cache[(size_t)c * a.B + sl[mb][h]] = v[mb][i];
+            }
+          } else {
+            const float h1 = stage[(SM::rH1 + c) * LD + trow[mb][h]];
+            v[mb][i] = (accA[mb][i] + sb0[c]) * (1.0f - h1 * h1);                                    // t1
           }
         }
-      } else {
-        float md[A];
+      wg_fence();
+      gemm2(accB, v, dW1T_hi, dW1T_lo, 4, MODE == MODE_FVP);          // H1 W1  |  += T1 W1
+      wg_commit();
+    }
+    float h2f[2][16];
+    if constexpr (MODE == MODE_FVP) {             // cached h2, requested while the GEMM runs
 #pragma unroll
-        for (int k = 0; k < A; ++k) md[k] = sbo[k];
+      for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-        for (int c = 0; c < H; ++c) {
-          colH2[c * LD] = h2[c];
-          const float t2 = (__uint_as_float(r[c]) + sb1[c]) * (1.0f - h2[c] * h2[c]);
+        for (int i = 0; i < 16; ++i)
+          h2f[mb][i] = a.h_cache[(size_t)(H + u_frag_col(i, lane)) * a.B + sl[mb][(i >> 1) & 1]];
+    }
+    wg_wait_all();
 #pragma unroll
-          for (int k = 0; k < A; ++k) md[k] = fmaf(t2, sWout[c * A + k], fmaf(h2[c], sVout[c * A + k], md[k]));
-        }
+    for (int mb = 0; mb < 2; ++mb) wg_fence_operand(accB[mb]);
+    // ================= E2 / E: second epilogue -> dmu, d2
+    {
+      float md[2][2][A];
 #pragma unroll
-        for (int k = 0; k < A; ++k) {
-          dmu[k] = valid ? md[k] * D.Mmu[k] : 0.f;
-          colDM[k * LD] = dmu[k];
-          colDL[k * LD] = 0.f;
+      for (int mb = 0; mb < 2; ++mb) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int k = 0; k < A; ++k) md[mb][h][k] = 0.f;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const int c = u_frag_col(i, lane), h = (i >> 1) & 1;
+          if constexpr (MODE != MODE_FVP) {
+            h2f[mb][i] = tanh_f(accB[mb][i] + sb1[c]);
+            if constexpr (MODE == MODE_GRAD) {
+              stage[(SM::rH2 + c) * LD + trow[mb][h]] = h2f[mb][i];
+              if (a.h_cache != nullptr && inrange[mb][h]) a.h_cache[(size_t)(H + c) * a.B + sl[mb][h]] = h2f[mb][i];
+            }
+#pragma unroll
+            for (int k = 0; k < A; ++k) md[mb][h][k] = fmaf(h2f[mb][i], sWout[c * A + k], md[mb][h][k]);
+          } else {
+            stage[(SM::rH2 + c) * LD + trow[mb][h]] = h2f[mb][i];
+            const float t2 = (accB[mb][i] + sb1[c]) * (1.0f - h2f[mb][i] * h2f[mb][i]);
+#pragma unroll
+            for (int k = 0; k < A; ++k)
+              md[mb][h][k] = fmaf(t2, sWout[c * A + k], fmaf(h2f[mb][i], sVout[c * A + k], md[mb][h][k]));
+          }
         }
       }
-      if constexpr (MODE != MODE_LOSS) {
-        float v[32];
+      // the four threads of a row (t4 = 0..3) hold disjoint column sets: combine
 #pragma unroll
-        for (int c = 0; c < H; ++c) {
-          float sacc = 0.f;
+      for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-          for (int k = 0; k < A; ++k) sacc = fmaf(dmu[k], sWout[c * A + k], sacc);
-          v[c] = sacc * (1.0f - h2[c] * h2[c]);
-          colD2[c * LD] = v[c];
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int k = 0; k < A; ++k) {
+            md[mb][h][k] += __shfl_xor_sync(0xffffffffu, md[mb][h][k], 1);
+            md[mb][h][k] += __shfl_xor_sync(0xffffffffu, md[mb][h][k], 2);
+          }
+      float dmu[2][2][A];
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = trow[mb][h];
+          if constexpr (MODE != MODE_FVP) {
+            float z[A], zsq = 0.f, zsq_old = 0.f, kl = 0.f;
+#pragma unroll
+            for (int k = 0; k < A; ++k) {
+              const float mu = sbo[k] + md[mb][h][k];
+              z[k] = (act[mb][h][k] - mu) * D.inv_std[k];
+              zsq += z[k] * z[k];
+              const float zo = (act[mb][h][k] - om[mb][h][k]) * D.inv_std_old[k];
+              zsq_old += zo * zo;
+              const float dm = om[mb][h][k] - mu;
+              kl += (dm * dm + D.var_old[k] - D.var_new[k]) / D.var_new2[k] + D.ls_new[k] - D.ls_old[k];
+            }
+            const float logp_new = -D.sum_ls_new - 0.5f * zsq - D.half_log2pi_A;
+            float w_s, term;
+            if (a.loss_kind == B200RL_LOSS_TRPO) {
+              const float logp_old = -D.sum_ls_old - 0.5f * zsq_old - D.half_log2pi_A;
+              w_s = expf(logp_new - logp_old) * adv_s[mb][h];
+              term = -w_s;
+            } else {
+              w_s = adv_s[mb][h];
+              term = -logp_new * adv_s[mb][h];
+            }
+            if (!valid[mb][h]) { w_s = 0.f; term = 0.f; }
+            if (t4 == 0) {
+              s_loss += (double)term;
+              if (valid[mb][h]) { s_kl += (double)kl; m_kl = fmax(m_kl, (double)kl); }
+            }
+            if constexpr (MODE == MODE_GRAD) {
+#pragma unroll
+              for (int k = 0; k < A; ++k) {
+                dmu[mb][h][k] = -w_s * z[k] * D.inv_std[k];
+                if (t4 == 0) {
+                  stage[(SM::rDM + k) * LD + r] = dmu[mb][h][k];
+                  stage[(SM::rDL + k) * LD + r] = -w_s * (z[k] * z[k] - 1.0f);
+                }
+              }
+            }
+          } else {
+#pragma unroll
+            for (int k = 0; k < A; ++k) {
+              dmu[mb][h][k] = valid[mb][h] ? (sbo[k] + md[mb][h][k]) * D.Mmu[k] : 0.f;
+              if (t4 == 0) {
+                stage[(SM::rDM + k) * LD + r] = dmu[mb][h][k];
+                stage[(SM::rDL + k) * LD + r] = 0.f;
+              }
+            }
+          }
         }
-        put_operand(v);
+      if constexpr (MODE != MODE_LOSS) {
+        float v[2][16];
+#pragma unroll
+        for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            const int c = u_frag_col(i, lane), h = (i >> 1) & 1;
+            float sacc = 0.f;
+#pragma unroll
+            for (int k = 0; k < A; ++k) sacc = fmaf(dmu[mb][h][k], sWout[c * A + k], sacc);
+            v[mb][i] = sacc * (1.0f - h2f[mb][i] * h2f[mb][i]);
+            stage[(SM::rD2 + c) * LD + trow[mb][h]] = v[mb][i];
+          }
+        wg_fence();
+        gemm2(accA, v, dW1_hi, dW1_lo, 4, false);                     // D2 W1^T
+        wg_commit();
       }
     }
     if constexpr (MODE != MODE_LOSS) {
-      u_fence_before();
-      __syncthreads();
-      if (tid == 0) {
-        u_fence_after();
-        split_gemm(SM::cACC_A, SM::cOP_HI, SM::cOP_LO, dW1_hi, dW1_lo, 4, false);               // D2 W1^T
-        u_commit(&bars[2]);
-      }
-      // (an L2 prefetch of the next tile's rows from here, as update_umma.cu does, was measured on Swimmer: 1.73 -> 1.77 ms)
+      __syncthreads();                       // stage rows of the whole tile written
       // ================= Gram part A behind the last GEMM: dW1 = H1^T D2, dWout, db1, dbout, dlog_std (tile_gram.cuh)
       gram.accumulate_a(stage, tid);
       __syncthreads();                       // every thread is done with the H2 rows: D1 may overwrite them
-      timed_out |= !u_wait(&bars[2], phase);
-      u_fence_after();
-      // ================= E3 / G: d1 = D1pre (1 - h1^2)
-      {
-        uint32_t r[32];
-        u_ld32(tlane + SM::cACC_A, r);
+      wg_wait_all();
 #pragma unroll
-        for (int c = 0; c < H; ++c) colD1[c * LD] = __uint_as_float(r[c]) * (1.0f - h1[c] * h1[c]);
-      }
-      u_fence_before();
+      for (int mb = 0; mb < 2; ++mb) wg_fence_operand(accA[mb]);
+      // ================= E3 / G: d1 = D1pre (1 - h1^2)
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const int c = u_frag_col(i, lane), r = trow[mb][(i >> 1) & 1];
+          const float h1 = stage[(SM::rH1 + c) * LD + r];
+          stage[(SM::rD1 + c) * LD + r] = accA[mb][i] * (1.0f - h1 * h1);
+        }
       __syncthreads();
       // ================= Gram part B: dW0 = X^T D1, db0
       gram.accumulate_b(stage, tid);
@@ -409,29 +396,23 @@ __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umm
   if constexpr (MODE != MODE_LOSS) {
     double* out = a.partial + (size_t)blockIdx.x * P;
     gram.write(out, reinterpret_cast<double*>(stage), tid);
-    __syncthreads();
-    if (timed_out) out[tid % P] = __longlong_as_double(0x7FF8000000000000ll);   // an MMA never completed: poison the result
-  } else if (timed_out) {
-    s_loss = __longlong_as_double(0x7FF8000000000000ll);
   }
   if constexpr (MODE != MODE_FVP) {
     // per-block (loss, sum KL | max KL): after the [grid][P] partial vectors (GRAD) or alone (LOSS), as loss_thread_kernel
+    if constexpr (MODE == MODE_GRAD) __syncthreads();
     double v[2] = {s_loss, s_kl};
     double mx[1] = {m_kl};
     double* sc = a.partial + (MODE == MODE_GRAD ? (size_t)gridDim.x * P : (size_t)0) + (size_t)blockIdx.x * 3;
     block_reduce_store<2, false>(v, red_scratch, sc);
     block_reduce_store<1, true>(mx, red_scratch, sc + 2);
   }
-  u_fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tbase), "r"(SM::TMEM_COLS));
 }
 
 template <class N, int MODE>
 static int launch_umma32(const UpdArgs& a, int* grid_out, cudaStream_t st) {
   using SM = Umma32<N, MODE>;
   B200RL_SET_MAX_SMEM((update_umma32_kernel<N, MODE>), SM::bytes);
-  long long grid = (long long)num_sms() * SM::MINB;        // persistent: every CTA resident, with its TMEM columns
+  long long grid = (long long)num_sms() * SM::MINB;        // persistent: every CTA resident
   const long long ntiles = host_n_tiles(a, V_TILE);
   if (grid > ntiles) grid = ntiles;
   if (grid > MAX_PARTIAL_BLOCKS) grid = MAX_PARTIAL_BLOCKS;

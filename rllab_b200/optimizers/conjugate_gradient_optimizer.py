@@ -10,7 +10,7 @@ line-search trial.
 
 Hessian-vector products (hvp_approach=):
   None / PerlmutterHvp()      exact product of the Hessian of mean KL = Gauss-Newton / Fisher product (:22-55).
-                              The float32 b200rl_fvp kernels (precision="f32", tcgen05) or the float64 parity kernels
+                              The float32 b200rl_fvp kernels (precision="f32", tensor cores) or the float64 parity kernels
                               (precision="f64").  NOTE: the reference's product is float64; on ill-conditioned Fisher systems
                               the float32 product costs the 10-iteration CG solve about three iterations of depth, which
                               shows in the learning speed of Swimmer (DESIGN.md section 5) -- raise cg_iters or use

@@ -1,7 +1,7 @@
 """Multi-GPU plumbing: one process per GPU (torchrun), lanes sharded by rank, all-reduce of the small float64 reduction
 vectors (gradient, FVP, loss/KL scalars, advantage statistics, baseline normal equations) over NVLink/NVSwitch.
 
-torch.distributed (NCCL) is the rendezvous and the fallback transport.  The data path on a B200 box is the library's own
+torch.distributed (NCCL) is the rendezvous and the fallback transport.  The data path on a multi-GPU box is the library's own
 peer-memory exchange (csrc/peer.cuh): every rank maps every other rank's exchange window (CUDA IPC), and one kernel per
 reduction pushes the vector through NVLink into all windows and folds the `world` copies in rank order -- fused into the
 finalize kernel of the policy-update passes (gradient, Fisher-vector product, loss/KL), stand-alone for the statistics

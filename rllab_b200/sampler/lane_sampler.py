@@ -1,4 +1,4 @@
-"""LaneSampler: the B200 replacement of BatchSampler + BaseSampler.process_samples
+"""LaneSampler: the GPU replacement of BatchSampler + BaseSampler.process_samples
 (rllab/algos/batch_polopt.py:9-34, rllab/sampler/base.py:40-182), plugged in through the reference's own
 `sampler_cls=` hook (batch_polopt.py:61-62,101-105).
 

@@ -2,7 +2,7 @@
 precisions -- the curves are chaotic (a 1e-16 perturbation moves the iteration-40 return by several units), so single runs
 say little.  Variants: f32 (shipped path), f64 (precision="f64" parity kernels), hilo (float32 kernels, CG direction split
 into two float32 words, two kernel calls), f64cg6 (float64 kernels, 6 CG iterations), f32cg20 (float32, 20 CG iterations).
-Usage: python scripts/exp_seed_sweep.py <n_seeds> [variants comma separated] [swimmer|hopper] -> gpurun_out/r02_seed_sweep_<env>.json"""
+Usage: python scripts/exp_seed_sweep.py <n_seeds> [variants comma separated] [swimmer|hopper] -> results/seed_sweep_<env>.json"""
 import json
 import os
 import sys
@@ -71,8 +71,8 @@ def main():
         tails = np.array([np.mean(r[-5:]) for r in out[v].values()])
         print("== %-8s last-5 mean over %d seeds: %.2f +- %.2f  (min %.2f max %.2f)" %
               (v, n, tails.mean(), tails.std(), tails.min(), tails.max()), flush=True)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    json.dump(out, open(os.path.join(ROOT, "gpurun_out", "r02_seed_sweep_%s.json" % env_name), "w"))
+    os.makedirs(os.path.join(ROOT, "results"), exist_ok=True)
+    json.dump(out, open(os.path.join(ROOT, "results", "seed_sweep_%s.json" % env_name), "w"))
 
 
 if __name__ == "__main__":

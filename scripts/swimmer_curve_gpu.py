@@ -1,6 +1,6 @@
 """GPU side of north_star's Swimmer learning check: TRPO on the device with the configuration of
 tests/golden/oracle_swimmer_trpo_curve.json (same lanes, horizon, Philox seed, policy seed), AverageReturn per iteration
-printed next to the float64 oracle's curve.  Run on a B200:  python scripts/swimmer_curve_gpu.py [n_itr] [swimmer|hopper]
+printed next to the float64 oracle's curve.  Run on an H100:  python scripts/swimmer_curve_gpu.py [n_itr] [swimmer|hopper]
 
 Iteration 0 sees the same initial policy and the same noise as the oracle run, so its AverageReturn must agree to the
 planar-dynamics tolerance; later iterations are two independent stochastic-optimisation trajectories of the same

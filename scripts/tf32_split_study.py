@@ -1,7 +1,7 @@
 """Accuracy of TF32 tensor-core formulations of the policy GEMMs, emulated in NumPy (no GPU needed).
 
 Question for the tensor-core update kernels (DESIGN.md section 8): which operand split keeps the float32-grade accuracy
-the parity tests need?  tcgen05 kind::tf32 reads 32-bit operands and keeps sign + 8 exponent + 10 mantissa bits
+the parity tests need?  wgmma .tf32 reads 32-bit operands and keeps sign + 8 exponent + 10 mantissa bits
 (truncation), products are exact, accumulation is float32.  Variants:
   1xTF32        a_hi*b_hi
   3xTF32        a_hi*b_hi + a_lo*b_hi + a_hi*b_lo          (lo = x - hi, itself truncated to tf32)

@@ -1,5 +1,5 @@
-"""tcgen05 Fisher-vector kernel (update_umma.cu) against the FP32 tiled-GEMM kernel and the float64 oracle on Hopper-shaped
-data, then timing at the cfg4 batch size.  Usage (under gpurun): timeout 300 python scripts/umma_fvp_check.py"""
+"""Tensor-core (wgmma) Fisher-vector kernel (update_umma.cu) against the FP32 tiled-GEMM kernel and the float64 oracle on Hopper-shaped
+data, then timing at the cfg4 batch size.  Usage: python scripts/umma_fvp_check.py"""
 import os
 import sys
 
@@ -50,7 +50,7 @@ def main():
         ref = P.fvp(theta, batch, xd.float().double().cpu().numpy(), dims, 0.0) + 1e-5 * x
         eu = np.abs(H_umma.cpu().numpy() - ref).max() / np.abs(ref).max()
         eg = np.abs(H_gemm.cpu().numpy() - ref).max() / np.abs(ref).max()
-        print("O=%d A=%d B=%d: max err / max|ref|  tcgen05 %.3e   FP32 GEMM %.3e   nan=%s" %
+        print("O=%d A=%d B=%d: max err / max|ref|  wgmma %.3e   FP32 GEMM %.3e   nan=%s" %
               (O, A, N * T, eu, eg, bool(np.isnan(H_umma.cpu().numpy()).any())), flush=True)
         if not (eu < 2e-4):
             ok = False
@@ -69,7 +69,7 @@ def main():
     ops.grad(L.LOSS_TRPO, th32, dd, 1e-6, b, g, None, hc)
     xd = torch.randn(dims.P, dtype=torch.float64, device=dev)
     out = torch.zeros_like(g)
-    for name, cache in (("tcgen05 (cached activations)", hc), ("FP32 tiled GEMM (no cache)", None)):
+    for name, cache in (("wgmma (cached activations)", hc), ("FP32 tiled GEMM (no cache)", None)):
         for _ in range(2):
             ops.fvp(th32, dd, 1e-6, b, xd, 1e-5, 1.0, out, cache)
         torch.cuda.synchronize()

@@ -429,7 +429,7 @@ def _check_update_kernels(dev, env_name, hidden, N, T):
     Hx_c = torch.zeros(dims.P, dtype=torch.float64, device=dev)
     ops.fvp(th32, dd, 1e-6, b, xd, 1e-5, 1.0, Hx_c, hc)
     # with a cache the dense chain runs on the tensor cores (update_umma32.cu / update_umma.cu: three-pass TF32 split,
-    # float32 accumulation in TMEM): float32-grade agreement with the FFMA kernel, not bit equality -- and the same
+    # float32 accumulation): float32-grade agreement with the FFMA kernel, not bit equality -- and the same
     # agreement with the float64 oracle as the FFMA kernel
     if True:
         np.testing.assert_allclose(Hx_c.cpu().numpy(), Hx.cpu().numpy(), rtol=0, atol=5e-6 * np.abs(Hx.cpu().numpy()).max())
