@@ -304,12 +304,15 @@ __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umm
         for (int h = 0; h < 2; ++h) {
           const int r = trow[mb][h];
           if constexpr (MODE != MODE_FVP) {
-            float z[A], zsq = 0.f, zsq_old = 0.f, kl = 0.f;
+            // z^2 is rounded on its own (__fmul_rn): the gradient pass reuses it for dlog_std, and a product that is free
+            // to contract into zsq's add would make the loss of the two modes differ in the last bit for A > 1
+            float z[A], zz[A], zsq = 0.f, zsq_old = 0.f, kl = 0.f;
 #pragma unroll
             for (int k = 0; k < A; ++k) {
               const float mu = sbo[k] + md[mb][h][k];
               z[k] = (act[mb][h][k] - mu) * D.inv_std[k];
-              zsq += z[k] * z[k];
+              zz[k] = __fmul_rn(z[k], z[k]);
+              zsq += zz[k];
               const float zo = (act[mb][h][k] - om[mb][h][k]) * D.inv_std_old[k];
               zsq_old += zo * zo;
               const float dm = om[mb][h][k] - mu;
@@ -336,7 +339,7 @@ __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umm
                 dmu[mb][h][k] = -w_s * z[k] * D.inv_std[k];
                 if (t4 == 0) {
                   stage[(SM::rDM + k) * LD + r] = dmu[mb][h][k];
-                  stage[(SM::rDL + k) * LD + r] = -w_s * (z[k] * z[k] - 1.0f);
+                  stage[(SM::rDL + k) * LD + r] = -w_s * (zz[k] - 1.0f);
                 }
               }
             }
