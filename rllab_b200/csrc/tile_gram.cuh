@@ -182,15 +182,20 @@ struct TileGram {
     for (int i = 0; i <= OQ; ++i) accB[i] += (double)sa[i];
   }
 
-  // out: this block's partial vector [P]; scr: >= 2 * 64 * 16 doubles of shared memory no thread still reads
+  // out: this block's partial vector [P]; scr: >= 2 * 64 * 16 doubles of shared memory no thread still reads;
+  // sync: the barrier of the 128 threads (__syncthreads, or a warpgroup's named barrier when a CTA holds several)
   __device__ __forceinline__ void write(double* out, double* scr, int tid) {
+    write(out, scr, tid, [] { __syncthreads(); });
+  }
+  template <class Sync>
+  __device__ __forceinline__ void write(double* out, double* scr, int tid, Sync sync) {
     const int w1_tile = tid & 63, kh = tid >> 6;
     const int ti = w1_tile >> 3, tj = w1_tile & 7;
 #pragma unroll
     for (int r = 0; r < 4; ++r)
 #pragma unroll
       for (int c = 0; c < 4; ++c) scr[(kh * 64 + w1_tile) * 16 + r * 4 + c] = accW1[r][c];
-    __syncthreads();
+    sync();
     if (tid < 64) {
 #pragma unroll
       for (int r = 0; r < 4; ++r)

@@ -38,9 +38,6 @@ constexpr int V_THREADS = 128, V_TILE = 128, V_LD = V_TILE + 4;
 #ifndef B200RL_V_PACKED_GRAM
 #define B200RL_V_PACKED_GRAM 1          // dW1 Gram with even / odd packed partial sums (tile_gram.cuh)
 #endif
-#ifndef B200RL_V_MAXB
-#define B200RL_V_MAXB 2                 // resident CTAs per SM of the gradient / Fisher passes: at three (168 registers)
-#endif                                  // the gradient pass spills
 
 template <class N, int MODE>
 struct Umma32 {
@@ -60,15 +57,64 @@ struct Umma32 {
   // (the forward-only loss pass stages nothing)
   static constexpr int rX = 0, rH1 = rX + O, rH2 = rH1 + H, rD1 = rH2, rD2 = rH2 + H, rDM = rD2 + H, rDL = rDM + A,
                        R = (MODE == MODE_LOSS) ? 0 : rDL + A;
-  static constexpr int o_red = ((o_stage + R * V_LD * 4 + 15) / 16) * 16;   // 3 x 32 doubles of reduction scratch
-  static constexpr size_t bytes = (size_t)o_red + 3 * 32 * 8;
+  // input ring: two slots of RR rows (pitch LD) -- obs[o], then (GRAD / LOSS) act[k], old_mean[k], adv -- filled by
+  // cp.async one tile ahead of the warpgroup that reads them
+  static constexpr int RR = O + (MODE == MODE_FVP ? 0 : 2 * A + 1), qX = 0, qAct = O, qOm = O + A, qAdv = O + 2 * A;
+  // every warpgroup owns one region: stage rows, 3 x 32 doubles of reduction scratch, input ring
+  static constexpr int w_red = ((R * V_LD * 4 + 15) / 16) * 16, w_ring = w_red + 3 * 32 * 8,
+                       w_bytes = w_ring + 2 * RR * V_LD * 4;
+  static constexpr int o_wg = ((o_stage + 15) / 16) * 16;
   static_assert(MODE == MODE_LOSS || 2 * 64 * 16 * 8 <= R * V_LD * 4, "stage region must hold the K-half combine scratch");
+  // warpgroups of the one CTA per SM: registers (64 K / 128 per warpgroup) and shared memory (227 KB; the images and
+  // small parameters are staged once per CTA).  Three (168 registers) for the loss pass and for the gradient pass of
+  // act_dim 1; two for the gradient pass of act_dim 2 / 3 (at 168 registers it spills) and for the Fisher pass (240+
+  // registers).  Every shape fits its count in shared memory.
+  static constexpr int NWG = (MODE == MODE_LOSS || (MODE == MODE_GRAD && A == 1)) ? 3 : 2;
+  static constexpr size_t bytes = (size_t)o_wg + (size_t)NWG * w_bytes;
   static_assert(bytes <= 232448, "does not fit the 227 KB of shared memory");
-  // resident CTAs per SM: shared memory (228 KB, 1 KB reserved per CTA), registers (64 K / 128 threads)
-  static constexpr int by_smem = (int)((228 * 1024) / (bytes + 1024));
-  static constexpr int cap = (MODE == MODE_LOSS) ? 3 : B200RL_V_MAXB;
-  static constexpr int MINB = by_smem < cap ? (by_smem < 1 ? 1 : by_smem) : cap;
 };
+
+// named barrier of one warpgroup (id 0 is __syncthreads)
+__device__ __forceinline__ void v_wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory"); }
+
+// one warpgroup's fixed-order reduction of K per-thread values, stored to out[0..K) (block_reduce_store for 128 threads)
+template <int K, bool IS_MAX>
+__device__ __forceinline__ void v_wg_reduce_store(const double (&v)[K], double* scratch, double* out, int tid, int wg) {
+  const int lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    double s = IS_MAX ? warp_max(v[k]) : warp_sum(v[k]);
+    if (lane == 0) scratch[k * 32 + warp] = s;
+  }
+  v_wg_sync(wg);
+  if (warp == 0) {
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+      double s = lane < 4 ? scratch[k * 32 + lane] : (IS_MAX ? -1.0e300 : 0.0);
+      s = IS_MAX ? warp_max(s) : warp_sum(s);
+      if (lane == 0) out[k] = s;
+    }
+  }
+  v_wg_sync(wg);
+}
+
+// request the ring rows of `tile` into `slot`: thread t copies sample t of every row (clamped to the last sample of the
+// batch, as the reads of a partial tile are), 4 B cp.async each (a row starts anywhere when B is not a multiple of 4)
+template <class SMT>
+__device__ __forceinline__ void v_ring_load(const UpdArgs& a, float* ring, int slot, long long tile, int tid) {
+  long long s = tile * V_TILE + tid;
+  if (s >= a.B) s = a.B - 1;
+  float* dst = ring + (size_t)slot * SMT::RR * V_LD + tid;
+#pragma unroll
+  for (int q = 0; q < SMT::RR; ++q) {
+    const float* src = q < SMT::qAct ? a.obs + (size_t)q * a.B + s
+                       : q < SMT::qOm ? a.act + (size_t)(q - SMT::qAct) * a.B + s
+                       : q < SMT::qAdv ? a.old_mean + (size_t)(q - SMT::qOm) * a.B + s
+                                       : a.adv + s;
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(u_smem_u32(dst + q * V_LD)), "l"(src) : "memory");
+  }
+  asm volatile("cp.async.commit_group;" ::: "memory");
+}
 
 // element (n, k) of a K-major [32 x K] image, byte offset (k: input feature, stored at u_kperm(k))
 __device__ __forceinline__ int v_boff(int n, int k) {
@@ -77,20 +123,24 @@ __device__ __forceinline__ int v_boff(int n, int k) {
 }
 
 template <class N, int MODE>
-__global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umma32_kernel(UpdArgs a) {
+__global__ void __launch_bounds__(V_THREADS * Umma32<N, MODE>::NWG, 1) update_umma32_kernel(UpdArgs a) {
   using SM = Umma32<N, MODE>;
   constexpr int O = N::O, H = 32, A = N::A, P = N::P, LD = V_LD, KX = SM::KX, KSX = KX / 8;
   extern __shared__ __align__(1024) unsigned char smem[];
   float* small = reinterpret_cast<float*>(smem + SM::o_small);
   float* sb0 = small, *sb1 = small + H, *sWout = small + 2 * H, *sVout = sWout + H * A;   // sVout: FVP only
   float* sbo = (MODE == MODE_FVP) ? sVout + H * A : sWout + H * A;
-  float* stage = reinterpret_cast<float*>(smem + SM::o_stage);
-  double* red_scratch = reinterpret_cast<double*>(smem + SM::o_red);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, t4 = lane & 3;
+  constexpr int NWG = SM::NWG, NT = NWG * V_THREADS;
+  // warpgroup wg works on its own tiles with its own stage rows and ring; tid, warp: inside the warpgroup
+  const int gtid = threadIdx.x, wg = gtid >> 7, tid = gtid & (V_THREADS - 1), warp = tid >> 5, lane = tid & 31, t4 = lane & 3;
+  unsigned char* wreg = smem + SM::o_wg + (size_t)wg * SM::w_bytes;
+  float* stage = reinterpret_cast<float*>(wreg);
+  double* red_scratch = reinterpret_cast<double*>(wreg + SM::w_red);
+  float* ring = reinterpret_cast<float*>(wreg + SM::w_ring);
 
   // ---- one-time setup: operand images of the weights, small parameters
   // MODE_GRAD: the chain multiplies by theta (params); MODE_FVP: first layers by the tangent x (xvec), W1 by theta
-  for (int e = tid; e < H * H; e += V_THREADS) {
+  for (int e = gtid; e < H * H; e += NT) {
     const int i = e / H, j = e % H;                                         // W1[i][j] (row-major in theta)
     const float w = a.params[N::oW1 + e];
     const float wh = tf32_hi(w);
@@ -107,7 +157,7 @@ __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umm
       *reinterpret_cast<float*>(smem + SM::o_bV1T + SM::IMG + v_boff(j, i)) = v - vh;
     }
   }
-  for (int e = tid; e < KX * H; e += V_THREADS) {
+  for (int e = gtid; e < KX * H; e += NT) {
     const int o = e / H, j = e % H;
     float v = 0.f;
     if (o < O) v = (MODE == MODE_FVP) ? (float)a.xvec[N::oW0 + o * H + j] : a.params[N::oW0 + o * H + j];
@@ -115,15 +165,15 @@ __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umm
     *reinterpret_cast<float*>(smem + SM::o_bXT + v_boff(j, o)) = vh;
     *reinterpret_cast<float*>(smem + SM::o_bXT + SM::IMGX + v_boff(j, o)) = v - vh;
   }
-  for (int e = tid; e < H * A; e += V_THREADS) {
+  for (int e = gtid; e < H * A; e += NT) {
     sWout[e] = a.params[N::oWo + e];
     if constexpr (MODE == MODE_FVP) sVout[e] = (float)a.xvec[N::oWo + e];
   }
-  for (int e = tid; e < H; e += V_THREADS) {
+  for (int e = gtid; e < H; e += NT) {
     sb0[e] = (MODE == MODE_FVP) ? (float)a.xvec[N::ob0 + e] : a.params[N::ob0 + e];
     sb1[e] = (MODE == MODE_FVP) ? (float)a.xvec[N::ob1 + e] : a.params[N::ob1 + e];
   }
-  if (tid < A) sbo[tid] = (MODE == MODE_FVP) ? (float)a.xvec[N::obo + tid] : a.params[N::obo + tid];
+  if (gtid < A) sbo[gtid] = (MODE == MODE_FVP) ? (float)a.xvec[N::obo + gtid] : a.params[N::obo + gtid];
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes of the images -> visible to wgmma
   __syncthreads();
 
@@ -150,9 +200,18 @@ __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umm
   if constexpr (MODE != MODE_LOSS) gram.init();
   double s_loss = 0.0, s_kl = 0.0, m_kl = -1.0e300;
 
-  const long long ntiles = n_tiles_of(a, V_TILE);
-  for (long long ti_ = blockIdx.x; ti_ < ntiles; ti_ += gridDim.x) {
+  // tiles go to the warpgroups of the grid round-robin: warpgroup vb takes tiles vb, vb + nvb, ...
+  const int ntiles = (int)n_tiles_of(a, V_TILE), nvb = gridDim.x * NWG, vb = blockIdx.x * NWG + wg;
+  if (vb < ntiles) v_ring_load<SM>(a, ring, 0, tile_at(a, vb), tid);
+  int slot = 0;
+  for (int ti_ = vb; ti_ < ntiles; ti_ += nvb, slot ^= 1) {
     const long long tile = tile_at(a, ti_);
+    // this tile's ring rows have landed (every thread waits for its own copies, the barrier publishes them), and every
+    // thread is done with the other slot: the next tile's rows go there while this one computes
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    v_wg_sync(wg);
+    if (ti_ + nvb < ntiles) v_ring_load<SM>(a, ring, slot ^ 1, tile_at(a, ti_ + nvb), tid);
+    const float* rs = ring + (size_t)slot * SM::RR * V_LD;
     // the thread's four samples: rows trow[mb][h] of the tile
     int trow[2][2];
     long long sl[2][2];
@@ -178,7 +237,7 @@ __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umm
           const int o = u_frag_col(i, lane), h = (i >> 1) & 1;
           float x = 0.f;
           if (o < O) {
-            x = a.obs[(size_t)o * a.B + sl[mb][h]];
+            x = rs[(SM::qX + o) * LD + trow[mb][h]];
             if constexpr (MODE != MODE_LOSS) stage[(SM::rX + o) * LD + trow[mb][h]] = x;
           }
           xf[mb][i] = x;
@@ -202,21 +261,6 @@ __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umm
         gemm2(accA, xf, dXT_hi, dXT_lo, KSX, false);                  // X W0
         wg_commit();
       }
-    }
-    // GRAD / LOSS: the remaining per-sample inputs, requested while the first GEMM runs
-    float act[2][2][A], om[2][2][A], adv_s[2][2];
-    if constexpr (MODE != MODE_FVP) {
-#pragma unroll
-      for (int mb = 0; mb < 2; ++mb)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-          for (int k = 0; k < A; ++k) {
-            act[mb][h][k] = a.act[(size_t)k * a.B + sl[mb][h]];
-            om[mb][h][k] = a.old_mean[(size_t)k * a.B + sl[mb][h]];
-          }
-          adv_s[mb][h] = a.adv[sl[mb][h]];
-        }
     }
     wg_wait_all();
 #pragma unroll
@@ -304,29 +348,37 @@ __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umm
         for (int h = 0; h < 2; ++h) {
           const int r = trow[mb][h];
           if constexpr (MODE != MODE_FVP) {
+            // the remaining per-sample inputs, from the ring (no registers held across the GEMMs)
+            float act[A], om[A];
+#pragma unroll
+            for (int k = 0; k < A; ++k) {
+              act[k] = rs[(SM::qAct + k) * LD + r];
+              om[k] = rs[(SM::qOm + k) * LD + r];
+            }
+            const float adv_s = rs[SM::qAdv * LD + r];
             // z^2 is rounded on its own (__fmul_rn): the gradient pass reuses it for dlog_std, and a product that is free
             // to contract into zsq's add would make the loss of the two modes differ in the last bit for A > 1
             float z[A], zz[A], zsq = 0.f, zsq_old = 0.f, kl = 0.f;
 #pragma unroll
             for (int k = 0; k < A; ++k) {
               const float mu = sbo[k] + md[mb][h][k];
-              z[k] = (act[mb][h][k] - mu) * D.inv_std[k];
+              z[k] = (act[k] - mu) * D.inv_std[k];
               zz[k] = __fmul_rn(z[k], z[k]);
               zsq += zz[k];
-              const float zo = (act[mb][h][k] - om[mb][h][k]) * D.inv_std_old[k];
+              const float zo = (act[k] - om[k]) * D.inv_std_old[k];
               zsq_old += zo * zo;
-              const float dm = om[mb][h][k] - mu;
+              const float dm = om[k] - mu;
               kl += (dm * dm + D.var_old[k] - D.var_new[k]) / D.var_new2[k] + D.ls_new[k] - D.ls_old[k];
             }
             const float logp_new = -D.sum_ls_new - 0.5f * zsq - D.half_log2pi_A;
             float w_s, term;
             if (a.loss_kind == B200RL_LOSS_TRPO) {
               const float logp_old = -D.sum_ls_old - 0.5f * zsq_old - D.half_log2pi_A;
-              w_s = expf(logp_new - logp_old) * adv_s[mb][h];
+              w_s = expf(logp_new - logp_old) * adv_s;
               term = -w_s;
             } else {
-              w_s = adv_s[mb][h];
-              term = -logp_new * adv_s[mb][h];
+              w_s = adv_s;
+              term = -logp_new * adv_s;
             }
             if (!valid[mb][h]) { w_s = 0.f; term = 0.f; }
             if (t4 == 0) {
@@ -373,13 +425,24 @@ __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umm
       }
     }
     if constexpr (MODE != MODE_LOSS) {
-      __syncthreads();                       // stage rows of the whole tile written
-      // ================= Gram part A behind the last GEMM: dW1 = H1^T D2, dWout, db1, dbout, dlog_std (tile_gram.cuh)
-      gram.accumulate_a(stage, tid);
-      __syncthreads();                       // every thread is done with the H2 rows: D1 may overwrite them
-      wg_wait_all();
+      // at three warpgroups per SM the last GEMM completes before the Gram phase: behind it, its A operand (64
+      // registers) would stay live through part A; the other two warpgroups cover the wait.  At two, part A runs
+      // behind it.
+      constexpr bool wait_first = NWG >= 3;
+      if constexpr (wait_first) {
+        wg_wait_all();
 #pragma unroll
-      for (int mb = 0; mb < 2; ++mb) wg_fence_operand(accA[mb]);
+        for (int mb = 0; mb < 2; ++mb) wg_fence_operand(accA[mb]);
+      }
+      v_wg_sync(wg);                         // stage rows of the whole tile written
+      // ================= Gram part A: dW1 = H1^T D2, dWout, db1, dbout, dlog_std (tile_gram.cuh)
+      gram.accumulate_a(stage, tid);
+      v_wg_sync(wg);                         // every thread is done with the H2 rows: D1 may overwrite them
+      if constexpr (!wait_first) {
+        wg_wait_all();
+#pragma unroll
+        for (int mb = 0; mb < 2; ++mb) wg_fence_operand(accA[mb]);
+      }
       // ================= E3 / G: d1 = D1pre (1 - h1^2)
 #pragma unroll
       for (int mb = 0; mb < 2; ++mb)
@@ -389,25 +452,25 @@ __global__ void __launch_bounds__(V_THREADS, (Umma32<N, MODE>::MINB)) update_umm
           const float h1 = stage[(SM::rH1 + c) * LD + r];
           stage[(SM::rD1 + c) * LD + r] = accA[mb][i] * (1.0f - h1 * h1);
         }
-      __syncthreads();
+      v_wg_sync(wg);
       // ================= Gram part B: dW0 = X^T D1, db0
       gram.accumulate_b(stage, tid);
-      __syncthreads();
+      v_wg_sync(wg);
     }
   }
 
   if constexpr (MODE != MODE_LOSS) {
-    double* out = a.partial + (size_t)blockIdx.x * P;
-    gram.write(out, reinterpret_cast<double*>(stage), tid);
+    double* out = a.partial + (size_t)vb * P;
+    gram.write(out, reinterpret_cast<double*>(stage), tid, [wg] { v_wg_sync(wg); });
   }
   if constexpr (MODE != MODE_FVP) {
-    // per-block (loss, sum KL | max KL): after the [grid][P] partial vectors (GRAD) or alone (LOSS), as loss_thread_kernel
-    if constexpr (MODE == MODE_GRAD) __syncthreads();
+    // per-warpgroup (loss, sum KL | max KL): after the [nvb][P] partial vectors (GRAD) or alone (LOSS), as
+    // loss_thread_kernel
     double v[2] = {s_loss, s_kl};
     double mx[1] = {m_kl};
-    double* sc = a.partial + (MODE == MODE_GRAD ? (size_t)gridDim.x * P : (size_t)0) + (size_t)blockIdx.x * 3;
-    block_reduce_store<2, false>(v, red_scratch, sc);
-    block_reduce_store<1, true>(mx, red_scratch, sc + 2);
+    double* sc = a.partial + (MODE == MODE_GRAD ? (size_t)nvb * P : (size_t)0) + (size_t)vb * 3;
+    v_wg_reduce_store<2, false>(v, red_scratch, sc, tid, wg);
+    v_wg_reduce_store<1, true>(mx, red_scratch, sc + 2, tid, wg);
   }
 }
 
@@ -415,14 +478,14 @@ template <class N, int MODE>
 static int launch_umma32(const UpdArgs& a, int* grid_out, cudaStream_t st) {
   using SM = Umma32<N, MODE>;
   B200RL_SET_MAX_SMEM((update_umma32_kernel<N, MODE>), SM::bytes);
-  long long grid = (long long)num_sms() * SM::MINB;        // persistent: every CTA resident
+  long long grid = num_sms();                              // persistent: one CTA of NWG warpgroups per SM
   const long long ntiles = host_n_tiles(a, V_TILE);
-  if (grid > ntiles) grid = ntiles;
-  if (grid > MAX_PARTIAL_BLOCKS) grid = MAX_PARTIAL_BLOCKS;
+  if (grid > (ntiles + SM::NWG - 1) / SM::NWG) grid = (ntiles + SM::NWG - 1) / SM::NWG;
+  if (grid > MAX_PARTIAL_BLOCKS / SM::NWG) grid = MAX_PARTIAL_BLOCKS / SM::NWG;
   if (grid < 1) grid = 1;
-  update_umma32_kernel<N, MODE><<<(unsigned)grid, V_THREADS, SM::bytes, st>>>(a);
+  update_umma32_kernel<N, MODE><<<(unsigned)grid, V_THREADS * SM::NWG, SM::bytes, st>>>(a);
   B200RL_LAUNCH_CHECK("update_umma32_kernel");
-  *grid_out = (int)grid;
+  *grid_out = (int)grid * SM::NWG;                         // one partial vector (and loss triple) per warpgroup
   return 0;
 }
 
