@@ -136,6 +136,14 @@ int b200rl_process_samples(int obs_dim, int N, int T, const float* obs, const fl
                            int drop_cut_paths, float* adv, float* ret, float* base, double* sums_out, double* maxs_out,
                            double* ws, void* stream);
 
+/* b200rl_process_samples with a baseline the caller has already written into `base` [T][N] float32 (read only): the
+ * LinearFeatureBaseline predict is skipped, the GAE scan and the statistics are the same kernels.  Used by baselines
+ * predicted by their own kernels (GaussianMLPBaseline.predict, gaussian_mlp_baseline.py:38-40, via b200rl_vf_forward). */
+int b200rl_process_samples_base(int obs_dim, int N, int T, const float* obs, const float* rew, unsigned char* flags,
+                                const unsigned short* tstep, const float* base, double discount, double gae_lambda,
+                                int drop_cut_paths, float* adv, float* ret, double* sums_out, double* maxs_out,
+                                double* ws, void* stream);
+
 /* center_advantages / shift_advantages_to_positive (rllab/algos/util.py:7-12) in place over B samples, from the
  * (already all-reduced) sums/maxs of b200rl_process_samples; masked samples (flags, may be NULL) keep adv = 0. */
 int b200rl_center_advantages(float* adv, long long B, const unsigned char* flags, const double* sums,
@@ -208,6 +216,42 @@ int b200rl_update_f64(int mode, int loss_kind, const double* params_f64, int obs
                       const float* old_mean, const float* old_log_std, const unsigned char* flags, const double* x,
                       double scale, const double* count, double reg_coeff, double diag_scale, double* vec_out,
                       double* loss_out, double* ws, void* stream);
+
+/* ---- GaussianMLPRegressor, the value function of GaussianMLPBaseline (rllab/regressors/gaussian_mlp_regressor.py,
+ * rllab/baselines/gaussian_mlp_baseline.py).  Net: MLP(obs_dim -> h1 -> h2 -> 1), ReLU hidden units, no output
+ * nonlinearity, one state-independent log_std (rllab/core/network.py:36-81, lasagne_layers.py ParamLayer); the flat
+ * parameter layout is the policy's with act_dim = 1.  Compiled for obs_dim in {2, 3, 4, 6, 13, 20}, hidden (32,32).
+ * stats [2*obs_dim+2] float64 = [x_mean (O), x_std (O), y_mean, y_std], the regressor's normalisation constants. ---- */
+
+/* Number of regressor parameters P (including log_std) for (O, h1, h2); <0 if the shape is not compiled in. */
+long long b200rl_vf_num_params(int obs_dim, int h1, int h2);
+
+/* Normalisation constants of GaussianMLPRegressor.fit (gaussian_mlp_regressor.py:197-208): column means and population
+ * standard deviations (+1e-8) of obs [O][B] and y [B] over the samples not carrying B200RL_FLAG_MASKED (flags may be
+ * NULL), in float64 and in two passes.  acc [2O+3] float64.  stage 0: acc[0..O+1] = (sum x_o, sum y, count); stage 1:
+ * acc[O+2..2O+2] = sum (x_o - mean_o)^2, sum (y - mean_y)^2 around the means of acc[0..O+1]; stage 2: stats_out from
+ * acc; stage 3: all three.  Across GPUs: all-reduce acc[0..O+1] after stage 0 and acc[O+2..] after stage 1. */
+int b200rl_vf_norm_stats(int obs_dim, long long B, const float* obs, const float* y, const unsigned char* flags,
+                         int stage, double* acc, double* stats_out, double* ws, void* stream);
+
+/* Regressor mean on obs [O][B] (f_predict / the mean half of f_pdists, gaussian_mlp_regressor.py:168-169,225-231):
+ * out [B] float32 = mu((x - x_mean) / x_std), times y_std plus y_mean if denormalize != 0.  Every sample is written. */
+int b200rl_vf_forward(const float* params_f32, int obs_dim, int h1, int h2, long long B, const float* obs,
+                      const double* stats, int denormalize, float* out, void* stream);
+
+/* One evaluation of the regressor objective (f_opt / f_loss / f_penalized_loss of penalty_lbfgs_optimizer.py:50-77 and
+ * lbfgs_optimizer.py:34-48 on the loss and mean-KL expressions of gaussian_mlp_regressor.py:150-166):
+ * loss_out [3] = scale * (sum NLL, sum KL(old || new), max KL) over the valid samples (divided by *count when count is
+ * not NULL), with NLL and KL of the Gaussian N(mu(nx), exp(log_std)) in normalised space against ny = (y - y_mean) /
+ * y_std.  mu_old [B] float32: the normalised mean at theta_old (b200rl_vf_forward with denormalize = 0), old_log_std its
+ * log_std; mu_old == NULL: no trust region (KL = 0).  g_out [P] float64 (or NULL = forward only): gradient of
+ * scale * sum (NLL + penalty * KL); with learn_std == 0 the log_std slot is 0 (not a trainable parameter).
+ * Arithmetic as b200rl_grad: float32 per sample and inside a 128-sample tile, float64 above; deterministic.  Reduced over
+ * the ranks of the peer communicator inside the pass while b200rl_peer_fuse_updates(1) is in effect. */
+int b200rl_vf_loss_grad(const float* params_f32, int obs_dim, int h1, int h2, long long B, const float* obs,
+                        const float* y, const unsigned char* flags, const double* stats, const float* mu_old,
+                        float old_log_std, double penalty, int learn_std, double scale, const double* count,
+                        double* g_out, double* loss_out, double* ws, void* stream);
 
 /* Workspace size (float64 entries) sufficient for every reduction above on the current device. */
 long long b200rl_ws_doubles(void);

@@ -41,6 +41,8 @@ SIGNATURES = {
                                _P, _P, _P, _P, _P, _P, _P, _P]),
     "b200rl_process_samples": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, c_double, c_double, c_int, _P, _P, _P,
                                        _P, _P, _P, _P]),
+    "b200rl_process_samples_base": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, c_double, c_double, c_int, _P, _P,
+                                            _P, _P, _P, _P]),
     "b200rl_center_advantages": (c_int, [_P, _LL, _P, _P, _P, c_int, c_int, _P]),
     "b200rl_lfb_gram": (c_int, [c_int, _LL, _P, _P, _P, _P, _P, _P, _P]),
     "b200rl_lfb_solve": (c_int, [c_int, _P, c_double, _P, _P, _P]),
@@ -71,6 +73,11 @@ SIGNATURES = {
     "b200rl_peer_timeouts": (c_int, [POINTER(c_uint)]),
     "b200rl_reduce_ranks": (c_int, [_P, c_int, _LL, _LL, _P, _P]),
     "b200rl_planes_to_rows_f64": (c_int, [c_int, _LL, _P, _P, _P]),
+    "b200rl_vf_num_params": (_LL, [c_int, c_int, c_int]),
+    "b200rl_vf_norm_stats": (c_int, [c_int, _LL, _P, _P, _P, c_int, _P, _P, _P, _P]),
+    "b200rl_vf_forward": (c_int, [_P, c_int, c_int, c_int, _LL, _P, _P, c_int, _P, _P]),
+    "b200rl_vf_loss_grad": (c_int, [_P, c_int, c_int, c_int, _LL, _P, _P, _P, _P, _P, c_float, c_double, c_int, c_double,
+                                    _P, _P, _P, _P, _P]),
 }
 
 _lib = None
@@ -139,4 +146,11 @@ def policy_num_params(O, h1, h2, A):
     n = load().b200rl_policy_num_params(O, h1, h2, A)
     if n < 0:
         raise B200RLError("unsupported policy network O=%d hidden=(%d,%d) A=%d: %s" % (O, h1, h2, A, last_error()))
+    return int(n)
+
+
+def vf_num_params(O, h1=32, h2=32):
+    n = load().b200rl_vf_num_params(O, h1, h2)
+    if n < 0:
+        raise B200RLError("unsupported regressor network O=%d hidden=(%d,%d): %s" % (O, h1, h2, last_error()))
     return int(n)

@@ -649,12 +649,11 @@ __global__ void planes_to_rows_kernel(int dim, long long B, const float* __restr
 
 using namespace b200rl;
 
-extern "C" {
-
-int b200rl_process_samples(int obs_dim, int N, int T, const float* obs, const float* rew, unsigned char* flags,
-                           const unsigned short* tstep, const double* w, double discount, double gae_lambda,
-                           int drop_cut_paths, float* adv, float* ret, float* base, double* sums_out, double* maxs_out,
-                           double* ws, void* stream) {
+// predict == false: `base` already holds the baseline of every sample (b200rl_process_samples_base)
+static int process_samples_impl(int obs_dim, int N, int T, const float* obs, const float* rew, unsigned char* flags,
+                                const unsigned short* tstep, const double* w, bool predict, double discount,
+                                double gae_lambda, int drop_cut_paths, float* adv, float* ret, float* base,
+                                double* sums_out, double* maxs_out, double* ws, void* stream) {
   B200RL_REQUIRE(obs && rew && flags && tstep && adv && ret && base && sums_out && maxs_out && ws,
                  "process_samples: null buffer");
   B200RL_REQUIRE(N > 0 && T > 0 && obs_dim > 0 && obs_dim <= OMAX, "process_samples: bad sizes");
@@ -664,7 +663,9 @@ int b200rl_process_samples(int obs_dim, int N, int T, const float* obs, const fl
   double* pmax = ws + (size_t)grid * B200RL_PS_NSUM;
   B200RL_REQUIRE((long long)grid * (B200RL_PS_NSUM + B200RL_PS_NMAX) <= b200rl_ws_doubles(), "workspace too small");
   const long long B = (long long)N * T;
-  if (w == nullptr) {                      // first iteration: the reference's baseline predicts zeros
+  if (!predict) {
+    // the caller filled `base` (a baseline other than LinearFeatureBaseline)
+  } else if (w == nullptr) {               // first iteration: the reference's baseline predicts zeros
     B200RL_CUDA_CHECK(cudaMemsetAsync(base, 0, (size_t)B * sizeof(float), st));
   } else {
     long long pg = (B / 4 + PRED_THREADS - 1) / PRED_THREADS;
@@ -694,6 +695,24 @@ int b200rl_process_samples(int obs_dim, int N, int T, const float* obs, const fl
   int rc = launch_finalize_sum(psum, grid, B200RL_PS_NSUM, sums_out, 1.0, st);
   if (rc) return rc;
   return launch_finalize_max(pmax, grid, B200RL_PS_NMAX, maxs_out, st);
+}
+
+extern "C" {
+
+int b200rl_process_samples(int obs_dim, int N, int T, const float* obs, const float* rew, unsigned char* flags,
+                           const unsigned short* tstep, const double* w, double discount, double gae_lambda,
+                           int drop_cut_paths, float* adv, float* ret, float* base, double* sums_out, double* maxs_out,
+                           double* ws, void* stream) {
+  return process_samples_impl(obs_dim, N, T, obs, rew, flags, tstep, w, true, discount, gae_lambda, drop_cut_paths, adv,
+                              ret, base, sums_out, maxs_out, ws, stream);
+}
+
+int b200rl_process_samples_base(int obs_dim, int N, int T, const float* obs, const float* rew, unsigned char* flags,
+                                const unsigned short* tstep, const float* base, double discount, double gae_lambda,
+                                int drop_cut_paths, float* adv, float* ret, double* sums_out, double* maxs_out,
+                                double* ws, void* stream) {
+  return process_samples_impl(obs_dim, N, T, obs, rew, flags, tstep, nullptr, false, discount, gae_lambda,
+                              drop_cut_paths, adv, ret, const_cast<float*>(base), sums_out, maxs_out, ws, stream);
 }
 
 int b200rl_center_advantages(float* adv, long long B, const unsigned char* flags, const double* sums,

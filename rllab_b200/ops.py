@@ -140,6 +140,46 @@ def process_samples(batch, w, discount, gae_lambda, drop_cut_paths=False):
     b.masked = bool(drop_cut_paths)
 
 
+def process_samples_base(batch, discount, gae_lambda, drop_cut_paths=False):
+    """process_samples with the baseline already in batch.base (GaussianMLPBaseline.predict_lanes)."""
+    b = batch
+    L.call("b200rl_process_samples_base", b.O, b.N, b.T, L.ptr(b.obs), L.ptr(b.rew), L.ptr(b.flags), L.ptr(b.tstep),
+           L.ptr(b.base), float(discount), float(gae_lambda), int(bool(drop_cut_paths)), L.ptr(b.adv), L.ptr(b.ret),
+           L.ptr(b.sums), L.ptr(b.maxs), L.ptr(workspace(b.device)), _stream())
+    b.masked = bool(drop_cut_paths)
+
+
+VF_STATS_SUMS, VF_STATS_SQUARES, VF_STATS_FINISH, VF_STATS_ALL = 0, 1, 2, 3
+
+
+def vf_norm_stats(O, B, obs, y, flags, stage, acc, stats_out):
+    """Regressor normalisation constants (b200rl_vf_norm_stats): acc [2O+3], stats_out [2O+2] float64."""
+    _chk(obs, F32, "obs", O * B), _chk(y, F32, "y", B), _chk(flags, U8, "flags", B)
+    _chk(acc, F64, "acc", 2 * O + 3), _chk(stats_out, F64, "stats_out", 2 * O + 2)
+    L.call("b200rl_vf_norm_stats", O, B, L.ptr(obs), L.ptr(y), L.ptr(flags), int(stage), L.ptr(acc), L.ptr(stats_out),
+           L.ptr(workspace(obs.device)), _stream())
+
+
+def vf_forward(params32, O, B, obs, stats, out, denormalize):
+    _chk(params32, F32, "params32", L.vf_num_params(O)), _chk(obs, F32, "obs", O * B)
+    _chk(stats, F64, "stats", 2 * O + 2), _chk(out, F32, "out", B)
+    L.call("b200rl_vf_forward", L.ptr(params32), O, 32, 32, B, L.ptr(obs), L.ptr(stats), int(bool(denormalize)),
+           L.ptr(out), _stream())
+
+
+def vf_loss_grad(params32, O, B, obs, y, flags, stats, mu_old, old_log_std, penalty, learn_std, scale, count, g_out,
+                 loss_out, fuse=False):
+    """loss_out[3] = (mean NLL, mean KL, max KL); g_out [P] (or None) = gradient of mean NLL + penalty * mean KL."""
+    P = L.vf_num_params(O)
+    _chk(params32, F32, "params32", P), _chk(obs, F32, "obs", O * B), _chk(y, F32, "y", B)
+    _chk(flags, U8, "flags", B), _chk(stats, F64, "stats", 2 * O + 2), _chk(mu_old, F32, "mu_old", B)
+    _chk(count, F64, "count", 1), _chk(g_out, F64, "g_out", P), _chk(loss_out, F64, "loss_out", 3)
+    with _Fused(fuse):
+        L.call("b200rl_vf_loss_grad", L.ptr(params32), O, 32, 32, B, L.ptr(obs), L.ptr(y), L.ptr(flags), L.ptr(stats),
+               L.ptr(mu_old), float(old_log_std), float(penalty), int(bool(learn_std)), float(scale), L.ptr(count),
+               L.ptr(g_out), L.ptr(loss_out), L.ptr(workspace(obs.device)), _stream())
+
+
 def _mask(batch):
     """(flags pointer, scale, count pointer) of an update pass over `batch`: with dropped paths the kernels skip
     FLAG_MASKED samples and divide by the device-resident valid-sample count; otherwise by B_global on the host."""

@@ -193,8 +193,17 @@ class LaneSampler(Sampler):
         from .. import ops
         algo = self.algo
         b = paths.lane_batch
-        w = algo.baseline.device_weights(b.O, b.device)
-        ops.process_samples(b, w, algo.discount, algo.gae_lambda, drop_cut_paths=bool(getattr(algo, "whole_paths", True)))
+        # a baseline with its own device predictor (GaussianMLPBaseline) writes batch.base itself; the previous fit's
+        # weights predict, the fit on this batch's returns follows the advantages (base.py:163-167)
+        own_predict = hasattr(algo.baseline, "predict_lanes")
+        if own_predict:
+            algo.baseline.predict_lanes(b)
+            ops.process_samples_base(b, algo.discount, algo.gae_lambda,
+                                     drop_cut_paths=bool(getattr(algo, "whole_paths", True)))
+        else:
+            w = algo.baseline.device_weights(b.O, b.device)
+            ops.process_samples(b, w, algo.discount, algo.gae_lambda,
+                                drop_cut_paths=bool(getattr(algo, "whole_paths", True)))
         # the baseline's normal equations only need the returns: reduce them right away so that ONE collective carries
         # the advantage sums, the normal equations and the maxima (the fit itself still follows the advantages, as in
         # base.py:163-167 -- the order has no numerical effect)
@@ -211,6 +220,8 @@ class LaneSampler(Sampler):
         logger.log("fitting baseline...")
         if lanes_fit:
             algo.baseline.solve_lanes(b)
+        elif own_predict:
+            algo.baseline.fit_lanes(b, self.comm)
         else:
             algo.baseline.fit(paths.to_paths())
         logger.log("fitted")
