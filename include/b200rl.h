@@ -189,6 +189,18 @@ int b200rl_grad(int loss_kind, const float* params_f32, int obs_dim, int h1, int
                 const float* old_log_std, const unsigned char* flags, double scale, const double* count, double* g_out,
                 double* loss_out, float* h_cache_out, double* ws, void* stream);
 
+/* Gradient of the penalised objective of PPO's L-BFGS step (penalty_lbfgs_optimizer.py:52-63 over the surrogate and
+ * mean KL of npo.py:72-82): g_out [P] float64 = scale * sum over valid samples of grad(surrogate_s + penalty * kl_s),
+ * kl_s = KL(old || new) of sample s, with the min_std mask of b200rl_grad on the log_std slot.  loss_out (3 doubles or
+ * NULL) receives the UNPENALISED triple (loss, sum kl, max kl) of the same pass, bit-identical to b200rl_grad's; the
+ * caller forms loss + penalty * mean kl in float64.  loss_kind: B200RL_LOSS_TRPO or B200RL_LOSS_VPG.  penalty >= 0 is applied in
+ * float32; penalty 0 runs b200rl_grad's pass (identical outputs).  Arguments otherwise as b200rl_grad (no activation
+ * cache).  Tensor-core kernels only: B200RL_EUNSUPPORTED in a B200RL_AB_TILE32 build. */
+int b200rl_grad_penalized(int loss_kind, double penalty, const float* params_f32, int obs_dim, int h1, int h2,
+                          int act_dim, float min_std, long long B, const float* obs, const float* act, const float* adv,
+                          const float* old_mean, const float* old_log_std, const unsigned char* flags, double scale,
+                          const double* count, double* g_out, double* loss_out, double* ws, void* stream);
+
 /* Fisher/Hessian-vector product of mean KL at theta_old (PerlmutterHvp, conjugate_gradient_optimizer.py:22-55):
  * Hx_out [P] = scale * sum_samples J^T M J x  (+ reg_coeff*x and the log_std block added once: pass
  * add_diag=1 on exactly one rank, or on all ranks with diag_scale = 1/world_size).  h_cache: activations written by

@@ -50,6 +50,8 @@ SIGNATURES = {
                                _P, _P, _P]),
     "b200rl_grad": (c_int, [c_int, _P, c_int, c_int, c_int, c_int, c_float, _LL, _P, _P, _P, _P, _P, _P, c_double, _P,
                             _P, _P, _P, _P, _P]),
+    "b200rl_grad_penalized": (c_int, [c_int, c_double, _P, c_int, c_int, c_int, c_int, c_float, _LL, _P, _P, _P, _P,
+                                      _P, _P, c_double, _P, _P, _P, _P, _P]),
     "b200rl_fvp": (c_int, [_P, c_int, c_int, c_int, c_int, c_float, _LL, _P, _P, _P, c_double, _P, c_double, c_double,
                            _P, _P, _P, c_int, _P, _P]),
     "b200rl_count_valid": (c_int, [_LL, _P, _P, c_int, _P, _P, _P]),

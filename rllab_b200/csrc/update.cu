@@ -184,6 +184,41 @@ int b200rl_grad(int loss_kind, const float* params_f32, int obs_dim, int h1, int
   return launch_finalize_update(f, st);
 }
 
+int b200rl_grad_penalized(int loss_kind, double penalty, const float* params_f32, int obs_dim, int h1, int h2,
+                          int act_dim, float min_std, long long B, const float* obs, const float* act, const float* adv,
+                          const float* old_mean, const float* old_log_std, const unsigned char* flags, double scale,
+                          const double* count, double* g_out, double* loss_out, double* ws, void* stream) {
+  B200RL_REQUIRE(params_f32 && obs && act && adv && old_mean && old_log_std && g_out && ws && B > 0,
+                 "grad_penalized: bad arguments");
+  B200RL_REQUIRE(loss_kind == B200RL_LOSS_TRPO || loss_kind == B200RL_LOSS_VPG, "grad_penalized: bad loss kind");
+  B200RL_REQUIRE(h1 == h2 && (h1 == 32 || h1 == 64), "grad_penalized: hidden sizes must be (32,32) or (64,64)");
+  B200RL_REQUIRE(penalty >= 0.0 && penalty <= 3.0e38, "grad_penalized: penalty must be finite and >= 0");
+#ifdef B200RL_AB_TILE32
+  (void)obs_dim; (void)act_dim; (void)min_std; (void)flags; (void)scale; (void)count; (void)loss_out; (void)stream;
+  set_error("grad_penalized: the KL-penalty mode exists only in the tensor-core kernels");
+  return B200RL_EUNSUPPORTED;
+#else
+  cudaStream_t st = (cudaStream_t)stream;
+  UpdArgs a{};
+  fill_args(a, params_f32, min_std, B, obs, act, adv, old_mean, old_log_std, loss_kind, flags, ws);
+  a.penalty = (float)penalty;
+  int grid = 0, P = 0, ols = 0;
+  // penalty 0 is the surrogate alone: the gradient pass itself, so that g_out is b200rl_grad's bit for bit on every net
+  // (the 64-wide KL-penalty instantiation is compiled on its own and need not round the surrogate terms identically)
+  const int mode = penalty == 0.0 ? MODE_GRAD : MODE_GRAD_KL;
+  int rc = (h1 == 32) ? update_umma32_launch(mode, obs_dim, act_dim, a, &grid, &P, &ols, st)
+                      : update_umma64_launch(mode, obs_dim, act_dim, a, &grid, &P, &ols, st);
+  if (rc) return rc;
+  FinArgs f{};
+  f.partial = ws; f.nblocks = grid; f.K = P; f.vec_out = g_out;
+  f.tri_partial = ws + (size_t)grid * P; f.NT = 3; f.tri_out = loss_out;
+  f.scale = scale; f.count = count; f.post = FIN_GRAD; f.ols = ols; f.A = act_dim;
+  f.params32 = params_f32; f.log_min_std = (double)a.log_min_std;
+  if (peer_fused()) f.peer = peer_next();
+  return launch_finalize_update(f, st);
+#endif
+}
+
 int b200rl_fvp(const float* params_f32, int obs_dim, int h1, int h2, int act_dim, float min_std, long long B,
                const float* obs, const unsigned char* flags, const double* x, double scale, const double* count,
                double reg_coeff, double diag_scale, double* Hx_out, const float* h_cache, const int* tile_list,

@@ -5,7 +5,10 @@
 
 namespace b200rl {
 
-constexpr int MODE_LOSS = 0, MODE_GRAD = 1, MODE_FVP = 2;
+// MODE_GRAD_KL: MODE_GRAD plus penalty * (gradient of the per-sample KL(old || new)), the objective of the penalised
+// L-BFGS policy update (tensor-core kernels only: update_umma.cu, update_umma32.cu)
+constexpr int MODE_LOSS = 0, MODE_GRAD = 1, MODE_FVP = 2, MODE_GRAD_KL = 3;
+constexpr bool is_grad_mode(int mode) { return mode == MODE_GRAD || mode == MODE_GRAD_KL; }
 
 struct UpdArgs {
   const float* params;
@@ -19,7 +22,23 @@ struct UpdArgs {
   const int* tile_list;        // FVP sub-sampling: indices of the 128-sample tiles to visit (device), or NULL = all tiles
   int n_list;
   double* partial;
+  float penalty;               // MODE_GRAD_KL only: weight of the KL term (after the other fields: their offsets stay)
 };
+
+// The KL-penalty terms of one valid sample and action dimension k, added to the surrogate's output deltas: the exact
+// derivatives of  kl_k = (dm^2 + var_old - var_new) / var_new2 + ls_new - ls_old,  dm = old_mean - mu,
+// var_new2 = 2 sigma^2 + 1e-8 (diagonal_gaussian.py:14-34), with respect to mu and log_std:
+//   dkl/dmu = -2 dm / var_new2,   dkl/dls = 1 - 2 sigma^2 (var_new2 + 2 num) / var_new2^2,   num = dm^2 + var_old - var_new
+// Every operation is rounded on its own, so no product of these terms contracts into the surrogate's arithmetic.
+__device__ __forceinline__ void add_kl_penalty(float pen, float dm, float var_new, float var_new2, float var_old,
+                                               float& dmu, float& dls) {
+  const float num = __fadd_rn(__fadd_rn(__fmul_rn(dm, dm), var_old), -var_new);
+  const float g_mu = __fdiv_rn(__fmul_rn(-2.0f, dm), var_new2);
+  const float t = __fmul_rn(__fmul_rn(2.0f, var_new), __fadd_rn(var_new2, __fmul_rn(2.0f, num)));
+  const float g_ls = __fadd_rn(1.0f, -__fdiv_rn(t, __fmul_rn(var_new2, var_new2)));
+  dmu = __fadd_rn(dmu, __fmul_rn(pen, g_mu));
+  dls = __fadd_rn(dls, __fmul_rn(pen, g_ls));
+}
 
 // valid sample: inside the batch and not masked out by process_samples(drop_cut_paths)
 __device__ __forceinline__ bool sample_valid(const UpdArgs& a, long long s) {

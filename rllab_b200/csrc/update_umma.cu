@@ -202,7 +202,7 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
     } else if (tid < H * A + A) {
       const int k = tid - H * A;
       out[N::obo + k] += (double)sum8(192 + k);
-    } else if (MODE == MODE_GRAD && tid < H * A + 2 * A) {
+    } else if (is_grad_mode(MODE) && tid < H * A + 2 * A) {
       const int k = tid - H * A - A;
       out[N::ols + k] += (double)sum8(196 + k);
     }
@@ -269,7 +269,7 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
     }
     // GRAD: the remaining per-sample inputs, requested while the first GEMM runs
     float act[2][A], om[2][A], adv_s[2] = {0.f, 0.f};
-    if constexpr (MODE == MODE_GRAD) {
+    if constexpr (is_grad_mode(MODE)) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
 #pragma unroll
@@ -351,7 +351,7 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
             dl[h][k] = 0.f;
           }
         } else {
-          float z[A], zsq = 0.f, zsq_old = 0.f, kl = 0.f;
+          float z[A], dmk[A], zsq = 0.f, zsq_old = 0.f, kl = 0.f;
 #pragma unroll
           for (int k = 0; k < A; ++k) {
             const float mu = svbo[k] + md[h][k];
@@ -360,6 +360,7 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
             const float zo = (act[h][k] - om[h][k]) * D.inv_std_old[k];
             zsq_old += zo * zo;
             const float dm = om[h][k] - mu;
+            dmk[k] = dm;
             kl += (dm * dm + D.var_old[k] - D.var_new[k]) / D.var_new2[k] + D.ls_new[k] - D.ls_old[k];
           }
           const float logp_new = -D.sum_ls_new - 0.5f * zsq - D.half_log2pi_A;
@@ -381,6 +382,9 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
           for (int k = 0; k < A; ++k) {
             dmu[h][k] = -w_s * z[k] * D.inv_std[k];
             dl[h][k] = -w_s * (z[k] * z[k] - 1.0f);
+            if constexpr (MODE == MODE_GRAD_KL) {
+              if (valid[h]) add_kl_penalty(a.penalty, dmk[k], D.var_new[k], D.var_new2[k], D.var_old[k], dmu[h][k], dl[h][k]);
+            }
           }
         }
       }
@@ -434,7 +438,7 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
       for (int k = 0; k < A; ++k) {
         const float sdm = warp_sum(t4 == 0 ? dmu[0][k] + dmu[1][k] : 0.f);
         if (lane == 0) gbo[k] += sdm;
-        if constexpr (MODE == MODE_GRAD) {
+        if constexpr (is_grad_mode(MODE)) {
           const float sdl = warp_sum(t4 == 0 ? dl[0][k] + dl[1][k] : 0.f);
           if (lane == 0) gls[k] += sdl;
         }
@@ -515,7 +519,7 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
     }
   }
   if (since_flush > 0) flush();
-  if constexpr (MODE == MODE_GRAD) {
+  if constexpr (is_grad_mode(MODE)) {
     __syncthreads();
     double v[2] = {s_loss, s_kl};
     double mx[1] = {m_kl};
@@ -545,8 +549,9 @@ int update_umma64_launch(int mode, int obs_dim, int act_dim, const UpdArgs& a, i
   B200RL_DISPATCH_NET_H(64, {
     *P_out = NetT::P;
     *ols_out = NetT::ols;
-    int rc = (mode == MODE_GRAD) ? launch_umma<NetT, MODE_GRAD>(a, grid_out, st)
-                                 : launch_umma<NetT, MODE_FVP>(a, grid_out, st);
+    int rc = (mode == MODE_GRAD)      ? launch_umma<NetT, MODE_GRAD>(a, grid_out, st)
+             : (mode == MODE_GRAD_KL) ? launch_umma<NetT, MODE_GRAD_KL>(a, grid_out, st)
+                                      : launch_umma<NetT, MODE_FVP>(a, grid_out, st);
     if (rc) return rc;
   });
   return 0;

@@ -69,7 +69,7 @@ struct Umma32 {
   // small parameters are staged once per CTA).  Three (168 registers) for the loss pass and for the gradient pass of
   // act_dim 1; two for the gradient pass of act_dim 2 / 3 (at 168 registers it spills) and for the Fisher pass (240+
   // registers).  Every shape fits its count in shared memory.
-  static constexpr int NWG = (MODE == MODE_LOSS || (MODE == MODE_GRAD && A == 1)) ? 3 : 2;
+  static constexpr int NWG = (MODE == MODE_LOSS || (is_grad_mode(MODE) && A == 1)) ? 3 : 2;
   static constexpr size_t bytes = (size_t)o_wg + (size_t)NWG * w_bytes;
   static_assert(bytes <= 232448, "does not fit the 227 KB of shared memory");
 };
@@ -278,7 +278,7 @@ __global__ void __launch_bounds__(V_THREADS * Umma32<N, MODE>::NWG, 1) update_um
           const int c = u_frag_col(i, lane), h = (i >> 1) & 1;
           if constexpr (MODE != MODE_FVP) {
             v[mb][i] = tanh_f(accA[mb][i] + sb0[c]);
-            if constexpr (MODE == MODE_GRAD) {
+            if constexpr (is_grad_mode(MODE)) {
               stage[(SM::rH1 + c) * LD + trow[mb][h]] = v[mb][i];
               if (a.h_cache != nullptr && inrange[mb][h]) a.h_cache[(size_t)c * a.B + sl[mb][h]] = v[mb][i];
             }
@@ -316,7 +316,7 @@ __global__ void __launch_bounds__(V_THREADS * Umma32<N, MODE>::NWG, 1) update_um
           const int c = u_frag_col(i, lane), h = (i >> 1) & 1;
           if constexpr (MODE != MODE_FVP) {
             h2f[mb][i] = tanh_f(accB[mb][i] + sb1[c]);
-            if constexpr (MODE == MODE_GRAD) {
+            if constexpr (is_grad_mode(MODE)) {
               stage[(SM::rH2 + c) * LD + trow[mb][h]] = h2f[mb][i];
               if (a.h_cache != nullptr && inrange[mb][h]) a.h_cache[(size_t)(H + c) * a.B + sl[mb][h]] = h2f[mb][i];
             }
@@ -358,7 +358,7 @@ __global__ void __launch_bounds__(V_THREADS * Umma32<N, MODE>::NWG, 1) update_um
             const float adv_s = rs[SM::qAdv * LD + r];
             // z^2 is rounded on its own (__fmul_rn): the gradient pass reuses it for dlog_std, and a product that is free
             // to contract into zsq's add would make the loss of the two modes differ in the last bit for A > 1
-            float z[A], zz[A], zsq = 0.f, zsq_old = 0.f, kl = 0.f;
+            float z[A], zz[A], dmk[A], zsq = 0.f, zsq_old = 0.f, kl = 0.f;
 #pragma unroll
             for (int k = 0; k < A; ++k) {
               const float mu = sbo[k] + md[mb][h][k];
@@ -368,6 +368,7 @@ __global__ void __launch_bounds__(V_THREADS * Umma32<N, MODE>::NWG, 1) update_um
               const float zo = (act[k] - om[k]) * D.inv_std_old[k];
               zsq_old += zo * zo;
               const float dm = om[k] - mu;
+              dmk[k] = dm;
               kl += (dm * dm + D.var_old[k] - D.var_new[k]) / D.var_new2[k] + D.ls_new[k] - D.ls_old[k];
             }
             const float logp_new = -D.sum_ls_new - 0.5f * zsq - D.half_log2pi_A;
@@ -385,11 +386,19 @@ __global__ void __launch_bounds__(V_THREADS * Umma32<N, MODE>::NWG, 1) update_um
               s_loss += (double)term;
               if (valid[mb][h]) { s_kl += (double)kl; m_kl = fmax(m_kl, (double)kl); }
             }
-            if constexpr (MODE == MODE_GRAD) {
+            if constexpr (is_grad_mode(MODE)) {
 #pragma unroll
               for (int k = 0; k < A; ++k) {
                 dmu[mb][h][k] = -w_s * z[k] * D.inv_std[k];
-                if (t4 == 0) {
+                if constexpr (MODE == MODE_GRAD_KL) {
+                  float dls = -w_s * (zz[k] - 1.0f);
+                  if (valid[mb][h])
+                    add_kl_penalty(a.penalty, dmk[k], D.var_new[k], D.var_new2[k], D.var_old[k], dmu[mb][h][k], dls);
+                  if (t4 == 0) {
+                    stage[(SM::rDM + k) * LD + r] = dmu[mb][h][k];
+                    stage[(SM::rDL + k) * LD + r] = dls;
+                  }
+                } else if (t4 == 0) {
                   stage[(SM::rDM + k) * LD + r] = dmu[mb][h][k];
                   stage[(SM::rDL + k) * LD + r] = -w_s * (zz[k] - 1.0f);
                 }
@@ -468,7 +477,7 @@ __global__ void __launch_bounds__(V_THREADS * Umma32<N, MODE>::NWG, 1) update_um
     // loss_thread_kernel
     double v[2] = {s_loss, s_kl};
     double mx[1] = {m_kl};
-    double* sc = a.partial + (MODE == MODE_GRAD ? (size_t)nvb * P : (size_t)0) + (size_t)vb * 3;
+    double* sc = a.partial + (is_grad_mode(MODE) ? (size_t)nvb * P : (size_t)0) + (size_t)vb * 3;
     v_wg_reduce_store<2, false>(v, red_scratch, sc, tid, wg);
     v_wg_reduce_store<1, true>(mx, red_scratch, sc + 2, tid, wg);
   }
@@ -495,9 +504,10 @@ int update_umma32_launch(int mode, int obs_dim, int act_dim, const UpdArgs& a, i
   B200RL_DISPATCH_NET_H(32, {
     *P_out = NetT::P;
     *ols_out = NetT::ols;
-    int rc = (mode == MODE_GRAD)   ? launch_umma32<NetT, MODE_GRAD>(a, grid_out, st)
-             : (mode == MODE_LOSS) ? launch_umma32<NetT, MODE_LOSS>(a, grid_out, st)
-                                   : launch_umma32<NetT, MODE_FVP>(a, grid_out, st);
+    int rc = (mode == MODE_GRAD)      ? launch_umma32<NetT, MODE_GRAD>(a, grid_out, st)
+             : (mode == MODE_GRAD_KL) ? launch_umma32<NetT, MODE_GRAD_KL>(a, grid_out, st)
+             : (mode == MODE_LOSS)    ? launch_umma32<NetT, MODE_LOSS>(a, grid_out, st)
+                                      : launch_umma32<NetT, MODE_FVP>(a, grid_out, st);
     if (rc) return rc;
   });
   return 0;

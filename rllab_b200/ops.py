@@ -255,6 +255,19 @@ def grad(loss_kind, params32, dims, min_std, batch, g_out, loss_out=None, h_cach
                L.ptr(h_cache), L.ptr(workspace(b.device)), _stream())
 
 
+def grad_penalized(loss_kind, penalty, params32, dims, min_std, batch, g_out, loss_out=None, fuse=False):
+    """g_out = gradient of surrogate + penalty * mean KL(old || new); loss_out[3] = the unpenalised (loss, mean KL,
+    max KL) of the same pass (b200rl_grad_penalized)."""
+    O, h1, h2, A = dims
+    b = batch
+    fl, scale, cnt = _mask(b)
+    _chk(params32, F32, "params32"), _chk(g_out, F64, "g_out")
+    with _Fused(fuse):
+        L.call("b200rl_grad_penalized", loss_kind, float(penalty), L.ptr(params32), O, h1, h2, A, float(min_std or 0.0),
+               b.B, L.ptr(b.obs), L.ptr(b.act), L.ptr(b.adv), L.ptr(b.mean), L.ptr(b.log_std), fl, scale, cnt,
+               L.ptr(g_out), L.ptr(loss_out), L.ptr(workspace(b.device)), _stream())
+
+
 def fvp(params32, dims, min_std, batch, x, reg_coeff, diag_scale, Hx_out, h_cache=None, tile_list=None, count=None,
         fuse=False):
     """tile_list (int32 device tensor) + count (float64 device scalar: valid samples in those tiles over all ranks):

@@ -38,6 +38,12 @@ class LbfgsOptimizer(object):
         self._target = target
         self._opt_fun = dict(f_loss=loss, f_opt=f_opt)
 
+    def __getstate__(self):
+        # snapshots drop the bound callables and target: the owner binds them again (VPG.init_opt on resume)
+        d = dict(self.__dict__)
+        d.update(_opt_fun=None, _target=None)
+        return d
+
     def loss(self, inputs, extra_inputs=None):
         if extra_inputs is None:
             extra_inputs = list()

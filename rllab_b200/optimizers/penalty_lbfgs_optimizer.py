@@ -63,6 +63,13 @@ class PenaltyLbfgsOptimizer(object):
         self._constraint_name = constraint_name
         self._opt_fun = dict(f_loss=loss, f_constraint=constraint_term, f_penalized_loss=f_penalized_loss, f_opt=f_opt)
 
+    def __getstate__(self):
+        # snapshots keep the carried penalty and drop the bound callables and target: the owner binds them again
+        # (NPO.init_opt on resume)
+        d = dict(self.__dict__)
+        d.update(_opt_fun=None, _target=None)
+        return d
+
     def loss(self, inputs):
         return self._opt_fun["f_loss"](*inputs)
 
