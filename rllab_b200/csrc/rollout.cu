@@ -64,31 +64,18 @@ struct RolloutArgs {
   float* log_std_out;
 };
 
-// Policy weights of the 32-wide rollout through the CONSTANT bank: with theta in a __constant__ array the dense layers
-// compile to FFMAs with a constant-bank operand (one load per warp, no LSU traffic) instead of LDS.128 + vector registers
-// (the fully unrolled 32-wide layers index the weights with compile-time offsets).  The thread-per-sample update
-// kernels keep theta in shared memory: their staging wants the registers.  theta is refreshed by one
-// stream-ordered device-to-device cudaMemcpyToSymbolAsync (<= 7 KB) per rollout.
-constexpr int ROLLOUT_CONST_MAXP = 2048;     // >= P of the largest 32-wide net (Hopper obs 20: 1 830)
-__constant__ __align__(16) float c_theta[ROLLOUT_CONST_MAXP];
-template <int H>
-constexpr bool rollout_const_weights() { return H == 32; }
-
 // One thread per lane; the whole T-step trajectory of a lane stays in that thread's registers.
 template <class Env, int H>
 __global__ void __launch_bounds__(ROLLOUT_THREADS, rollout_minblocks<Env, H>()) rollout_kernel(RolloutArgs a) {
   using N_ = Net<Env::O, H, H, Env::A>;
-  // 32-wide: parameters in the constant bank; 64-wide: parameters in shared memory + one activation column per thread
-  // for the rolled layer-2 loop
+  // parameters in shared memory: the dense layers read every weight with a broadcast LDS.128 (all threads of the warp
+  // load the same address); 64-wide: + one activation column per thread for the rolled layer-2 loop
   constexpr int P4 = (N_::P + 3) & ~3;
-  constexpr bool CW = rollout_const_weights<H>();
   extern __shared__ __align__(16) float rollout_smem[];
-  const float* sp = CW ? c_theta : rollout_smem;
+  const float* sp = rollout_smem;
   float* hcol = (H > 32) ? rollout_smem + P4 + threadIdx.x : nullptr;
-  if constexpr (!CW) {
-    for (int i = threadIdx.x; i < N_::P; i += blockDim.x) rollout_smem[i] = a.params[i];
-    __syncthreads();
-  }
+  for (int i = threadIdx.x; i < N_::P; i += blockDim.x) rollout_smem[i] = a.params[i];
+  __syncthreads();
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   float std_[Env::A];
 #pragma unroll
@@ -237,10 +224,8 @@ static int launch_rollout(int h, const RolloutArgs& a, cudaStream_t st) {
   const int grid = (a.N + ROLLOUT_THREADS - 1) / ROLLOUT_THREADS;
   if (h == 32) {
     using N32 = Net<Env::O, 32, 32, Env::A>;
-    static_assert(N32::P <= ROLLOUT_CONST_MAXP, "constant bank too small for this net");
-    B200RL_CUDA_CHECK(cudaMemcpyToSymbolAsync(c_theta, a.params, (size_t)N32::P * sizeof(float), 0,
-                                              cudaMemcpyDeviceToDevice, st));
-    rollout_kernel<Env, 32><<<grid, ROLLOUT_THREADS, 0, st>>>(a);
+    const size_t smem = ((N32::P + 3) & ~3) * sizeof(float);
+    rollout_kernel<Env, 32><<<grid, ROLLOUT_THREADS, smem, st>>>(a);
   } else if (h == 64) {
     using N64 = Net<Env::O, 64, 64, Env::A>;
     const size_t smem = (((N64::P + 3) & ~3) + 64 * ROLLOUT_THREADS) * sizeof(float);
