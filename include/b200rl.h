@@ -318,6 +318,42 @@ int b200rl_peer_fuse_updates(int enable);
  * Synchronising device->host read: call it at the end of a job, not inside the iteration. */
 int b200rl_peer_timeouts(unsigned int* count_out_host);
 
+/* ---- Cross-entropy method (rllab/algos/cem.py): a population of policies, one parameter row per member. ---- */
+
+/* Parameter rows of CEM._worker_rollout_policy (cem.py:30-36, `np.random.standard_normal(K) * sample_std + cur_mean`):
+ * theta_out [n][P] float64, row r = member m_r = members[r] (device int64 list) or member0 + r (members NULL):
+ * theta[r][k] = cur_mean[k] + sample_std[k] * eps(seed, iter, m_r, k), sample_std[k] = sqrt(cur_std[k]^2 + extra_var)
+ * (cem.py:117-118 with extra_var = extra_std^2 * max(1 - itr / extra_decay_time, 0)).  eps is Philox stream 2 (lane = m,
+ * row 0, chunk k / 4) through the normal map of b200rl_fill_noise; every float64 operation is explicitly rounded, so the
+ * same arithmetic in NumPy on the same eps gives the same bits.  Rows are a pure function of (seed, iter, m, cur_mean,
+ * cur_std, extra_var): a rank can regenerate any member's row. */
+int b200rl_population_sample(long long P, const double* cur_mean, const double* cur_std, double extra_var,
+                             unsigned int seed, unsigned int iter, const long long* members, long long member0, int n,
+                             double* theta_out, void* stream);
+
+/* n_evals episodes of each of M policies (cem.py:37-57 over rollout, rllab/sampler/utils.py:6-43): member m's policy is
+ * row m of theta [M][P] float64 (rounded to float32 when staged).  Every episode starts from reset and runs to done or
+ * max_path_length (no auto-reset, nothing per step written); episode (m, e) uses lane lane0 + m*n_evals + e for its
+ * action and reset noise and is bit-identical to the first path of lane e of b200rl_rollout(theta_m as float32,
+ * N = n_evals, lane0 = lane0 + m*n_evals, same seed / iter).  Outputs [M][n_evals]: ret_out = discounted return
+ * (discount_cumsum(rewards, discount)[0], float64 accumulated in the kernel), undisc_out = sum of rewards, len_out = episode
+ * length; obs_first / obs_last [M][n_evals][O] (both NULL or both set) = the episode's first and last observation.
+ * member_out [M][3] = (fitness mean(ret) - std(ret, ddof)/sqrt(n_evals), the same statistic of undisc, mean over action
+ * dims of the member's action std exp(max(log_std, log(min_std)))), ddof = 1 if n_evals > 1 else 0 (cem.py:15-27).
+ * ws: workspace of b200rl_ws_doubles() entries (its first word is the persistent grid's work counter). */
+int b200rl_population_rollout(int env_kind, int h1, int h2, float min_std, const double* theta, int M, int n_evals,
+                              int max_path_length, double discount, unsigned int seed, unsigned int iter,
+                              long long lane0, double* ret_out, double* undisc_out, int* len_out, float* obs_first,
+                              float* obs_last, double* member_out, double* ws, void* stream);
+
+/* Elite indices of CEM.train (cem.py:138, `(-fs).argsort()[:n_best]`): idx_out [k] int64 = the indices of the k largest of
+ * f [M] float64 in descending order, ties to the lower index, NaN last; deterministic, no host sort.  k <= M. */
+int b200rl_population_topk(const double* f, int M, int k, long long* idx_out, double* ws, void* stream);
+
+/* cur_mean / cur_std of CEM.train (cem.py:140-141): mean_out, std_out [P] = column mean and population std (ddof 0) of
+ * rows [k][P] float64, summed over the rows in row order with explicitly rounded operations (NumPy's axis-0 reduction). */
+int b200rl_rows_mean_std(long long P, int k, const double* rows, double* mean_out, double* std_out, void* stream);
+
 /* (T,N)-planar lane layout <-> the reference's sample-major (B, dim) float64 wire format
  * (samples_data["observations"] etc., rllab/sampler/base.py:74-104): dst[(t*N+n)*dim + k] = src[k][t][n]. */
 int b200rl_planes_to_rows_f64(int dim, long long B, const float* src, double* dst, void* stream);

@@ -80,6 +80,11 @@ SIGNATURES = {
     "b200rl_vf_forward": (c_int, [_P, c_int, c_int, c_int, _LL, _P, _P, c_int, _P, _P]),
     "b200rl_vf_loss_grad": (c_int, [_P, c_int, c_int, c_int, _LL, _P, _P, _P, _P, _P, c_float, c_double, c_int, c_double,
                                     _P, _P, _P, _P, _P]),
+    "b200rl_population_sample": (c_int, [_LL, _P, _P, c_double, c_uint, c_uint, _P, _LL, c_int, _P, _P]),
+    "b200rl_population_rollout": (c_int, [c_int, c_int, c_int, c_float, _P, c_int, c_int, c_int, c_double, c_uint, c_uint,
+                                          _LL, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "b200rl_population_topk": (c_int, [_P, c_int, c_int, _P, _P, _P]),
+    "b200rl_rows_mean_std": (c_int, [_LL, c_int, _P, _P, _P, _P]),
 }
 
 _lib = None

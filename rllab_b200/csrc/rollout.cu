@@ -16,40 +16,6 @@ constexpr int ROLLOUT_THREADS = 128;
 template <class Env, int H>
 constexpr int rollout_minblocks() { return (H == 32 && Env::S <= 4) ? 4 : 1; }
 
-template <class Env>
-__device__ __forceinline__ void draw_reset(float (&s)[Env::S], const float* __restrict__ reset_raw, int row, int N,
-                                           int n, uint32_t seed, uint32_t iter, long long lane) {
-  float raw[Env::K];
-  if (reset_raw != nullptr) {
-#pragma unroll
-    for (int k = 0; k < Env::K; ++k) raw[k] = reset_raw[((size_t)row * Env::K + k) * N + n];
-  } else {
-#pragma unroll
-    for (int c = 0; c < (Env::K + 3) / 4; ++c) {
-      float q[4];
-      noise4(Env::NOISE, seed, iter, 1, lane, row, c, q);
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        if (c * 4 + i < Env::K) raw[c * 4 + i] = q[i];
-    }
-  }
-  Env::reset(s, raw);
-}
-
-template <int A>
-__device__ __forceinline__ void draw_eps(float (&e)[A], const float* __restrict__ eps, int row, long long N,
-                                         long long n, uint32_t seed, uint32_t iter, long long lane) {
-  if (eps != nullptr) {
-#pragma unroll
-    for (int a = 0; a < A; ++a) e[a] = eps[((size_t)row * A + a) * N + n];
-  } else {
-    float q[4];
-    noise4<(A + 1) / 2>(B200RL_NOISE_NORMAL, seed, iter, 0, lane, row, 0, q);
-#pragma unroll
-    for (int a = 0; a < A; ++a) e[a] = q[a];
-  }
-}
-
 struct RolloutArgs {
   const float* params;
   float log_min_std;

@@ -79,6 +79,11 @@ def set_snapshot_gap(g):
     _snapshot_gap = g
 
 
+def snapshot_enabled():
+    """True when save_itr_params writes a file (callers can skip building a snapshot's host copies otherwise)."""
+    return bool(_snapshot_dir) and _snapshot_mode != "none"
+
+
 def save_itr_params(itr, params):
     """rllab/misc/logger.py:216-232 (pickle instead of joblib.dump; same file names)."""
     if not _snapshot_dir or _snapshot_mode == "none":

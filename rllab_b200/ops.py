@@ -340,6 +340,67 @@ def planes_to_rows_f64(src, dim, B, dst):
     L.call("b200rl_planes_to_rows_f64", dim, B, L.ptr(src), L.ptr(dst), _stream())
 
 
+I64, I32 = torch.int64, torch.int32
+
+
+def population_sample(cur_mean, cur_std, extra_var, seed, it, theta_out, members=None, member0=0):
+    """theta_out [n][P] float64: CEM parameter rows of members `members` (int64 device tensor) or member0 .. member0+n-1."""
+    P = cur_mean.numel()
+    _chk(cur_mean, F64, "cur_mean"), _chk(cur_std, F64, "cur_std", P), _chk(members, I64, "members")
+    n = theta_out.shape[0]
+    _chk(theta_out, F64, "theta_out", n * P)
+    if members is not None and members.numel() != n:
+        raise ValueError("members must have one entry per row of theta_out")
+    L.call("b200rl_population_sample", P, L.ptr(cur_mean), L.ptr(cur_std), float(extra_var), int(seed) & 0xFFFFFFFF,
+           int(it) & 0xFFFFFFFF, L.ptr(members), int(member0), n, L.ptr(theta_out), _stream())
+
+
+class PopulationResult(object):
+    """Device outputs of one population rollout of M members x E evals (b200rl_population_rollout)."""
+
+    def __init__(self, M, E, O, device, keep_obs=True):
+        self.M, self.E, self.O = M, E, O
+        self.ret = torch.empty((M, E), dtype=F64, device=device)
+        self.undisc = torch.empty((M, E), dtype=F64, device=device)
+        self.len = torch.empty((M, E), dtype=I32, device=device)
+        self.obs_first = torch.empty((M, E, O), dtype=F32, device=device) if keep_obs else None
+        self.obs_last = torch.empty((M, E, O), dtype=F32, device=device) if keep_obs else None
+        self.member = torch.empty((M, 3), dtype=F64, device=device)
+
+
+def population_rollout(kind, theta, h1, h2, min_std, n_evals, max_path_length, discount, seed, it, lane0, out):
+    """out: PopulationResult with out.M == theta.shape[0]; lane0 = global lane of member 0, eval 0."""
+    M = theta.shape[0]
+    _chk(theta, F64, "theta")
+    if out.M != M or out.E != n_evals:
+        raise ValueError("result buffers are %d x %d, the call is %d x %d" % (out.M, out.E, M, n_evals))
+    info = L.env_info(kind)                                  # raises on an unknown env kind
+    if out.O != info["obs_dim"]:
+        raise ValueError("result buffers hold %d-dim observations, the env has %d" % (out.O, info["obs_dim"]))
+    if h1 == h2 and h1 in (32, 64):                          # other shapes are rejected by the library itself
+        P = L.policy_num_params(info["obs_dim"], h1, h2, info["act_dim"])
+        if theta.dim() != 2 or theta.shape[1] != P:
+            raise ValueError("theta must be [M][%d] for this env and net, got %s" % (P, tuple(theta.shape)))
+    L.call("b200rl_population_rollout", kind, h1, h2, float(min_std or 0.0), L.ptr(theta), M, n_evals,
+           int(max_path_length), float(discount), int(seed) & 0xFFFFFFFF, int(it) & 0xFFFFFFFF, int(lane0),
+           L.ptr(out.ret), L.ptr(out.undisc), L.ptr(out.len), L.ptr(out.obs_first), L.ptr(out.obs_last),
+           L.ptr(out.member), L.ptr(workspace(theta.device)), _stream())
+
+
+def population_topk(f, k, idx_out):
+    """idx_out [k] int64: indices of the k largest of f (float64), descending, ties to the lower index."""
+    _chk(f, F64, "f"), _chk(idx_out, I64, "idx_out", k)
+    L.call("b200rl_population_topk", L.ptr(f), f.numel(), int(k), L.ptr(idx_out), L.ptr(workspace(f.device)),
+           _stream())
+
+
+def rows_mean_std(rows, mean_out, std_out):
+    """Column mean / population std of rows [k][P] float64 in row order."""
+    k, P = rows.shape
+    _chk(rows, F64, "rows"), _chk(mean_out, F64, "mean_out", P), _chk(std_out, F64, "std_out", P)
+    L.call("b200rl_rows_mean_std", P, k, L.ptr(rows), L.ptr(mean_out), L.ptr(std_out), _stream())
+
+
 class PendingHost(object):
     """Asynchronous device->host readback of a small tensor: the copy into pinned host memory is queued on the current
     stream together with an event; `get()` waits for that event only (not for later work on the stream) and returns a

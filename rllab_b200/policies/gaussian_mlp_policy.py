@@ -112,6 +112,14 @@ class GaussianMLPPolicy(object):
         from .. import ops
         ops.f64_to_f32(self._theta64, self._theta32)  # value.astype(dtype), parameterized.py:68
 
+    def set_param_values_device(self, theta64):
+        """set_param_values from a float64 device tensor [P], without a host round trip (CEM's best row)."""
+        from .. import ops
+        th64, th32 = self._ensure_device()
+        th64.copy_(theta64.reshape(-1))
+        ops.f64_to_f32(th64, th32)
+        self.version += 1
+
     def get_param_shapes(self, **tags):
         return self._shapes()
 
