@@ -354,6 +354,27 @@ int b200rl_population_topk(const double* f, int M, int k, long long* idx_out, do
  * rows [k][P] float64, summed over the rows in row order with explicitly rounded operations (NumPy's axis-0 reduction). */
 int b200rl_rows_mean_std(long long P, int k, const double* rows, double* mean_out, double* std_out, void* stream);
 
+/* ---- Relative entropy policy search (rllab/algos/reps.py): the dual g(eta, v) over the lane batch. ----
+ * Sample (t, n) has the Bellman error delta = rew + (phi(t+1, n) - phi(t, n)) . v with the LinearFeatureBaseline feature
+ * map phi = [clip(o, +-10), o^2, al, al^2, al^3, 1], al = tstep / 100 (reps.py:207-211), and phi(t+1, n) = 0 when (t, n)
+ * carries B200RL_FLAG_END (the per-path feat_diff of reps.py:227-238, including a path cut by the end of the buffer).
+ * v [2*obs_dim+4] float64.  masked != 0: samples carrying B200RL_FLAG_MASKED are left out of the maximum and every sum.
+ * float64 arithmetic, two-stage fixed-order reductions (bit-identical reruns).  obs_dim in {2, 3, 4, 6, 13, 20}, else
+ * B200RL_EUNSUPPORTED.  Across GPUs: all-reduce out_max (max) before b200rl_reps_dual_sums, and `out` (sum) after it. */
+
+/* out_max[0] = M = max delta over this GPU's valid samples (the max(delta_v / eta) shift of reps.py:107,169-172). */
+int b200rl_reps_delta_max(int obs_dim, int N, int T, const float* obs, const float* rew, const unsigned char* flags,
+                          const unsigned short* tstep, int masked, const double* v, double* out_max, double* ws,
+                          void* stream);
+
+/* The sums behind the dual and its gradient (reps.py:164-187), with e = exp((delta - M) / eta) and M = *M (device):
+ * out [2*obs_dim+6] float64 = [sum e, sum e (delta - M), sum e feat_diff (2*obs_dim+4 entries)] over the valid samples.
+ * The caller forms g = eta eps + eta log(sum e / count) + M (+ L2 term) and its gradient from them.  w_out ([T][N] float32
+ * or NULL) receives e per sample (0 on masked samples): the weights of the policy loss of reps.py:110-112. */
+int b200rl_reps_dual_sums(int obs_dim, int N, int T, const float* obs, const float* rew, const unsigned char* flags,
+                          const unsigned short* tstep, int masked, const double* v, double eta, const double* M,
+                          double* out, float* w_out, double* ws, void* stream);
+
 /* (T,N)-planar lane layout <-> the reference's sample-major (B, dim) float64 wire format
  * (samples_data["observations"] etc., rllab/sampler/base.py:74-104): dst[(t*N+n)*dim + k] = src[k][t][n]. */
 int b200rl_planes_to_rows_f64(int dim, long long B, const float* src, double* dst, void* stream);

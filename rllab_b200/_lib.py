@@ -85,6 +85,8 @@ SIGNATURES = {
                                           _LL, _P, _P, _P, _P, _P, _P, _P, _P]),
     "b200rl_population_topk": (c_int, [_P, c_int, c_int, _P, _P, _P]),
     "b200rl_rows_mean_std": (c_int, [_LL, c_int, _P, _P, _P, _P]),
+    "b200rl_reps_delta_max": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, c_int, _P, _P, _P, _P]),
+    "b200rl_reps_dual_sums": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, c_int, _P, c_double, _P, _P, _P, _P, _P]),
 }
 
 _lib = None

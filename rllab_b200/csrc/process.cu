@@ -5,38 +5,34 @@
 //           rllab/baselines/linear_feature_baseline.py:19-43.
 // All three kernels are HBM-streaming (16-40 B per sample); sums are float64, two-stage, fixed order.
 #include "mlp.cuh"   // gram_4x4 (packed FFMA2 outer products); includes common.cuh
+#include "lfb_features.cuh"
 
 namespace b200rl {
 
 constexpr int OMAX = 32;  // max obs_dim handled by the runtime-O feature code
 
-// LinearFeatureBaseline features . w  (linear_feature_baseline.py:19-23): [clip(o,+-10), o^2, al, al^2, al^3, 1]
+// LinearFeatureBaseline features . w  (linear_feature_baseline.py:19-23, feature map in lfb_features.cuh)
 // OT > 0: compile-time obs_dim -- the O loads of a step are issued back to back (and, with the caller's step loop
 // unrolled, hoisted across steps) instead of one load -> use chain per feature (in-order issue stalls at the first use of
 // every load: the runtime-O loop exposed 8 x O serial DRAM latencies per window -- 0.55 ms on cfg2, round 2 measurement)
 template <int OT>
 __device__ __forceinline__ double lfb_predict(const float* __restrict__ obs, size_t plane, size_t idx, int O_rt,
                                               unsigned short ts, const double* __restrict__ w) {
-  double acc = 0.0;
-  const int O = OT > 0 ? OT : O_rt;
   if constexpr (OT > 0) {
     float ov[OT];
 #pragma unroll
     for (int k = 0; k < OT; ++k) ov[k] = obs[k * plane + idx];
-#pragma unroll
-    for (int k = 0; k < OT; ++k) {
-      const double o = (double)fminf(fmaxf(ov[k], -10.0f), 10.0f);
-      acc += o * w[k] + (o * o) * w[OT + k];
-    }
+    return lfb_dot<OT>(ov, ts, w);
   } else {
-    for (int k = 0; k < O; ++k) {
+    double acc = 0.0;
+    for (int k = 0; k < O_rt; ++k) {
       double o = (double)fminf(fmaxf(obs[k * plane + idx], -10.0f), 10.0f);
-      acc += o * w[k] + (o * o) * w[O + k];
+      acc += o * w[k] + (o * o) * w[O_rt + k];
     }
+    double al = (double)ts / 100.0;
+    acc += al * w[2 * O_rt] + (al * al) * w[2 * O_rt + 1] + (al * al * al) * w[2 * O_rt + 2] + w[2 * O_rt + 3];
+    return acc;
   }
-  double al = (double)ts / 100.0;
-  acc += al * w[2 * O] + (al * al) * w[2 * O + 1] + (al * al * al) * w[2 * O + 2] + w[2 * O + 3];
-  return acc;
 }
 
 // process_samples = two streaming kernels (round 2, second design; the block-cooperative time-parallel scan of the first
@@ -57,19 +53,6 @@ __device__ __forceinline__ double lfb_predict(const float* __restrict__ obs, siz
 // vectorized_sampler.py drops unfinished running_paths): its samples get FLAG_MASKED, adv = 0, and are excluded from
 // every statistic (count, path counts, returns); downstream kernels skip masked samples.
 constexpr int PRED_THREADS = 256;
-
-template <int OT>
-__device__ __forceinline__ double lfb_dot(const float (&ov)[OT > 0 ? OT : 1], unsigned short ts, const double* __restrict__ w) {
-  double acc = 0.0;
-#pragma unroll
-  for (int k = 0; k < OT; ++k) {
-    const double o = (double)fminf(fmaxf(ov[k], -10.0f), 10.0f);
-    acc += o * w[k] + (o * o) * w[OT + k];
-  }
-  const double al = (double)ts / 100.0;
-  acc += al * w[2 * OT] + (al * al) * w[2 * OT + 1] + (al * al * al) * w[2 * OT + 2] + w[2 * OT + 3];
-  return acc;
-}
 
 template <int OT>
 __global__ void __launch_bounds__(PRED_THREADS) lfb_predict_kernel(int O_rt, long long B, const float* __restrict__ obs,

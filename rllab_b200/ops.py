@@ -401,6 +401,25 @@ def rows_mean_std(rows, mean_out, std_out):
     L.call("b200rl_rows_mean_std", P, k, L.ptr(rows), L.ptr(mean_out), L.ptr(std_out), _stream())
 
 
+def reps_delta_max(batch, v, out_max):
+    """out_max[1] = max over this GPU's valid samples of the REPS Bellman error r + feat_diff . v (b200rl_reps_delta_max)."""
+    b = batch
+    _chk(v, F64, "v", 2 * b.O + 4), _chk(out_max, F64, "out_max", 1)
+    L.call("b200rl_reps_delta_max", b.O, b.N, b.T, L.ptr(b.obs), L.ptr(b.rew), L.ptr(b.flags), L.ptr(b.tstep),
+           int(bool(b.masked)), L.ptr(v), L.ptr(out_max), L.ptr(workspace(b.device)), _stream())
+
+
+def reps_dual_sums(batch, v, eta, M, out, w_out=None):
+    """out [2O+6] = [sum e, sum e (delta - M), sum e feat_diff] with e = exp((delta - M) / eta) over this GPU's valid
+    samples; w_out ([T][N] float32 or None) = e, 0 on masked samples (b200rl_reps_dual_sums).  M: float64 device [1]."""
+    b = batch
+    _chk(v, F64, "v", 2 * b.O + 4), _chk(M, F64, "M", 1), _chk(out, F64, "out", 2 * b.O + 6)
+    _chk(w_out, F32, "w_out", b.B)
+    L.call("b200rl_reps_dual_sums", b.O, b.N, b.T, L.ptr(b.obs), L.ptr(b.rew), L.ptr(b.flags), L.ptr(b.tstep),
+           int(bool(b.masked)), L.ptr(v), float(eta), L.ptr(M), L.ptr(out), L.ptr(w_out), L.ptr(workspace(b.device)),
+           _stream())
+
+
 class PendingHost(object):
     """Asynchronous device->host readback of a small tensor: the copy into pinned host memory is queued on the current
     stream together with an event; `get()` waits for that event only (not for later work on the stream) and returns a
