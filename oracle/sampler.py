@@ -170,15 +170,20 @@ def explained_variance_1d(ypred, y):
     return 1 - np.var(y - ypred) / (vary + 1e-8)
 
 
-def process_samples_lanes(traj, coeffs, discount, gae_lambda, center_adv=True, positive_adv=False, drop_cut=False):
+def process_samples_lanes(traj, coeffs, discount, gae_lambda, center_adv=True, positive_adv=False, drop_cut=False,
+                          base=None):
     """sampler/base.py:48-182 on the lane layout.  `coeffs` = LinearFeatureBaseline weights of the
     previous iteration (None -> zeros, linear_feature_baseline.py:41-42).  Returns dict with
     adv/ret/base (T,N) and the tabular statistics.  drop_cut: whole paths only (see valid_mask): the samples of cut
-    paths get adv = 0 and are left out of the centering and of every statistic; `valid` (T,N) is returned."""
+    paths get adv = 0 and are left out of the centering and of every statistic; `valid` (T,N) is returned.
+    `base` (T,N), if given, is the baseline of every sample (any baseline's predict) and `coeffs` is ignored; `und`
+    (T,N) is the undiscounted return-to-go."""
     rew = np.asarray(traj["rew"], np.float64)
     T, N = rew.shape
     ends = (traj["flags"] & FLAG_END) != 0
-    if coeffs is None:
+    if base is not None:
+        base = np.asarray(base, np.float64)
+    elif coeffs is None:
         base = np.zeros((T, N))
     else:
         F = lfb_features_lanes(traj["obs"], traj["tstep"])
@@ -229,7 +234,7 @@ def process_samples_lanes(traj, coeffs, discount, gae_lambda, center_adv=True, p
         MinReturn=float(np.min(undisc)),
         adv_mean=float(adv_mean), adv_std=float(adv_std),
     )
-    return dict(adv=adv_out, adv_raw=adv, ret=ret, base=base, stats=stats, valid=valid)
+    return dict(adv=adv_out, adv_raw=adv, ret=ret, und=und, base=base, stats=stats, valid=valid)
 
 
 def truncate_paths_lengths(lengths, max_samples):

@@ -4,7 +4,7 @@
 // Replaces: rllab/sampler/base.py:48-93,163-180 ; rllab/misc/special.py:51-59,107-111 ; rllab/algos/util.py:7-12 ;
 //           rllab/baselines/linear_feature_baseline.py:19-43.
 // All three kernels are HBM-streaming (16-40 B per sample); sums are float64, two-stage, fixed order.
-#include "mlp.cuh"   // gram_4x4 (packed FFMA2 outer products); includes common.cuh
+#include "common.cuh"
 #include "lfb_features.cuh"
 
 namespace b200rl {
@@ -499,8 +499,11 @@ __global__ void __launch_bounds__(128, 3) lfb_gram_reg_kernel(long long B, const
 // Larger observation spaces (obs_dim 6 / 13 / 20: DoublePendulum, Swimmer, Hopper): the d1 x d1 Gram (d1 = 2 O + 5 <= 45)
 // in 4x4 register tiles over the upper triangle, as tile_gram.cuh does for dW1: features of a 128-sample tile staged
 // feature-major in shared memory, thread = (tile of the upper triangle, K-slice of the 128 samples), 8 LDS.128 per 32
-// packed FFMA2, float32 inside a tile and float64 across tiles.  The pair-per-thread kernel above (kept for other
-// obs_dim) re-reads two whole rows per pair: 1.25 ms per Swimmer iteration against 0.3 ms here.
+// DFMA.  Features and products are float64 throughout (features computed in float64 from the float32 observations, as
+// the reference's featmat): these Grams are ill-conditioned (Hopper's o and o^2 columns are nearly collinear with the
+// constant), and a float32 Gram -- float32 features and float32 sums inside a tile -- moved Hopper's fitted baseline by
+// up to 5 % of max |ret| from the reference's lstsq and needed a regularisation retry (DESIGN.md section 5).  The
+// pair-per-thread kernel above (kept for other obs_dim) re-reads two whole rows per pair.
 template <int O>
 struct GramTile {
   static constexpr int D1 = 2 * O + 5, NB = (D1 + 3) / 4, NT = NB * (NB + 1) / 2;      // 4x4 tiles of the upper triangle
@@ -508,7 +511,7 @@ struct GramTile {
   static constexpr int PER = ((GRAM_TILE / KS + 3) / 4) * 4;                            // samples per slice (multiple of 4)
   static constexpr int ROWS = NB * 4;
   static_assert(NT <= GRAM_THREADS, "one thread per (tile, slice)");
-  static constexpr size_t tile_bytes = (size_t)ROWS * GRAM_LD * sizeof(float), scr_bytes = (size_t)KS * NT * 16 * 8;
+  static constexpr size_t tile_bytes = (size_t)ROWS * GRAM_LD * sizeof(double), scr_bytes = (size_t)KS * NT * 16 * 8;
   static constexpr size_t smem = tile_bytes > scr_bytes ? tile_bytes : scr_bytes;   // the slice-combine scratch reuses it
 };
 
@@ -519,7 +522,8 @@ __global__ void __launch_bounds__(GRAM_THREADS, 3)
                          double* __restrict__ partial) {
   using G = GramTile<O>;
   constexpr int D1 = G::D1, NB = G::NB, NP = D1 * (D1 + 1) / 2, LD = GRAM_LD;
-  extern __shared__ __align__(16) float F[];    // [ROWS][LD]; rows >= D1 stay zero
+  extern __shared__ __align__(16) double FD[];   // [ROWS][LD]; rows >= D1 stay zero (own name: F[] above is float)
+  double* F = FD;
   const int tid = threadIdx.x;
   // this thread's tile (bi <= bj) and K-slice
   const int tix = tid % G::NT, ks = tid / G::NT;
@@ -533,7 +537,7 @@ __global__ void __launch_bounds__(GRAM_THREADS, 3)
   for (int r = 0; r < 4; ++r)
 #pragma unroll
     for (int c = 0; c < 4; ++c) acc[r][c] = 0.0;
-  for (int i = tid; i < G::ROWS * LD; i += GRAM_THREADS) F[i] = 0.f;
+  for (int i = tid; i < G::ROWS * LD; i += GRAM_THREADS) F[i] = 0.0;
   const long long ntiles = (B + GRAM_TILE - 1) / GRAM_TILE;
   for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const long long sidx = tile * GRAM_TILE + tid;
@@ -542,44 +546,38 @@ __global__ void __launch_bounds__(GRAM_THREADS, 3)
       float ov[O];
 #pragma unroll
       for (int k = 0; k < O; ++k) ov[k] = obs[(size_t)k * B + sidx];
-      const float al = (float)tstep[sidx] / 100.0f, rt = ret[sidx];
+      const double al = (double)tstep[sidx] / 100.0;
 #pragma unroll
       for (int k = 0; k < O; ++k) {
-        const float o = fminf(fmaxf(ov[k], -10.0f), 10.0f);
+        const double o = (double)fminf(fmaxf(ov[k], -10.0f), 10.0f);
         F[k * LD + tid] = o;
         F[(O + k) * LD + tid] = o * o;
       }
       F[(2 * O) * LD + tid] = al;
       F[(2 * O + 1) * LD + tid] = al * al;
       F[(2 * O + 2) * LD + tid] = al * al * al;
-      F[(2 * O + 3) * LD + tid] = 1.0f;
-      F[(2 * O + 4) * LD + tid] = rt;
+      F[(2 * O + 3) * LD + tid] = 1.0;
+      F[(2 * O + 4) * LD + tid] = (double)ret[sidx];
     } else {
 #pragma unroll
-      for (int k = 0; k < D1; ++k) F[k * LD + tid] = 0.0f;
+      for (int k = 0; k < D1; ++k) F[k * LD + tid] = 0.0;
     }
     __syncthreads();
     if (worker) {
-      float2 a2[4][4];
-#pragma unroll
-      for (int r = 0; r < 4; ++r)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) a2[r][c] = make_float2(0.f, 0.f);
-      const float* U = F + (bi * 4) * LD;
-      const float* V = F + (bj * 4) * LD;
+      const double* U = F + (bi * 4) * LD;
+      const double* V = F + (bj * 4) * LD;
 #pragma unroll 2
-      for (int k = k_lo; k < k_hi; k += 4) {
-        float4 u[4], v[4];
+      for (int k = k_lo; k < k_hi; k += 2) {
+        double2 u[4], v[4];
 #pragma unroll
-        for (int r = 0; r < 4; ++r) u[r] = *reinterpret_cast<const float4*>(U + r * LD + k);
+        for (int r = 0; r < 4; ++r) u[r] = *reinterpret_cast<const double2*>(U + r * LD + k);
 #pragma unroll
-        for (int c = 0; c < 4; ++c) v[c] = *reinterpret_cast<const float4*>(V + c * LD + k);
-        gram_4x4(u, v, a2);
+        for (int c = 0; c < 4; ++c) v[c] = *reinterpret_cast<const double2*>(V + c * LD + k);
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+          for (int c = 0; c < 4; ++c) acc[r][c] = fma(u[r].y, v[c].y, fma(u[r].x, v[c].x, acc[r][c]));
       }
-#pragma unroll
-      for (int r = 0; r < 4; ++r)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) acc[r][c] += (double)(a2[r][c].x + a2[r][c].y);
     }
   }
   // combine the K-slices of a tile in fixed order through shared memory, then store the upper-triangle entries
@@ -611,7 +609,8 @@ template <int O>
 static int launch_gram_tile(long long B, const float* obs, const unsigned short* tstep, const float* ret,
                             const unsigned char* flags, double* ws, int* grid_out, cudaStream_t st) {
   using G = GramTile<O>;
-  static_assert(G::smem <= 48 * 1024, "default dynamic shared-memory limit");
+  static_assert(3 * G::smem <= 227 * 1024, "three CTAs per SM");
+  if (G::smem > 48 * 1024) B200RL_SET_MAX_SMEM(lfb_gram_tile_kernel<O>, G::smem);   // obs_dim 20: 49.5 KB
   long long g = (long long)num_sms() * 3;
   const long long ntiles = (B + GRAM_TILE - 1) / GRAM_TILE;
   if (g > ntiles) g = ntiles;
