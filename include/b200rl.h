@@ -47,6 +47,7 @@ extern "C" {
 #define B200RL_ENV_HOPPER 4
 #define B200RL_ENV_CARTPOLE_SWINGUP 5 /* rllab/envs/box2d/cartpole_swingup_env.py (same Box2D model as CartpoleEnv) */
 #define B200RL_ENV_DOUBLE_PENDULUM 6 /* rllab/envs/box2d/double_pendulum_env.py (models/double_pendulum.xml.mako) */
+#define B200RL_ENV_HALF_CHEETAH 7 /* rllab/envs/mujoco/half_cheetah_env.py (vendor/mujoco_models/half_cheetah.xml) */
 
 #define B200RL_NOISE_UNIFORM 0
 #define B200RL_NOISE_NORMAL 1

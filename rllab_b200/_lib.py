@@ -12,8 +12,10 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libb200rl.so")
 
 ENV_POINT, ENV_CARTPOLE, ENV_PENDULUM, ENV_SWIMMER, ENV_HOPPER, ENV_CARTPOLE_SWINGUP, ENV_DOUBLE_PENDULUM = 0, 1, 2, 3, 4, 5, 6
+ENV_HALF_CHEETAH = 7
 ENV_KINDS = dict(point=ENV_POINT, cartpole=ENV_CARTPOLE, pendulum=ENV_PENDULUM, swimmer=ENV_SWIMMER, hopper=ENV_HOPPER,
-                 cartpole_swingup=ENV_CARTPOLE_SWINGUP, double_pendulum=ENV_DOUBLE_PENDULUM)
+                 cartpole_swingup=ENV_CARTPOLE_SWINGUP, double_pendulum=ENV_DOUBLE_PENDULUM,
+                 half_cheetah=ENV_HALF_CHEETAH)
 NOISE_UNIFORM, NOISE_NORMAL = 0, 1
 LOSS_TRPO, LOSS_VPG, LOSS_KL = 0, 1, 2
 FLAG_DONE, FLAG_END, FLAG_CUT, FLAG_MASKED = 1, 2, 4, 8

@@ -3,6 +3,7 @@
 //   reset(s, raw) ; obs(s, o) ; step(s, u, r, done)   with u = action after NormalizedEnv scaling.
 // Reference classes are cited per struct; the NormalizedEnv action map lives in scale_action().
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 
 namespace b200rl {
@@ -197,7 +198,8 @@ namespace b200rl {
 #ifdef B200RL_HAVE_PLANAR
 #define B200RL_PLANAR_CASES(...)                                                              \
     case B200RL_ENV_SWIMMER: { using Env = ::b200rl::SwimmerEnvD; __VA_ARGS__; } break;       \
-    case B200RL_ENV_HOPPER: { using Env = ::b200rl::HopperEnvD; __VA_ARGS__; } break;
+    case B200RL_ENV_HOPPER: { using Env = ::b200rl::HopperEnvD; __VA_ARGS__; } break;       \
+    case B200RL_ENV_HALF_CHEETAH: { using Env = ::b200rl::HalfCheetahEnvD; __VA_ARGS__; } break;
 #else
 #define B200RL_PLANAR_CASES(...)
 #endif
@@ -225,7 +227,7 @@ __device__ __forceinline__ void draw_reset(float (&s)[Env::S], const float* __re
 }
 
 // Action noise of one lane at step `row`: eps [row][A][N] (tests) or Philox stream 0 at (lane, row).
-template <int A>
+template <int A, typename std::enable_if<(A <= 4), int>::type = 0>
 __device__ __forceinline__ void draw_eps(float (&e)[A], const float* __restrict__ eps, int row, long long N,
                                          long long n, uint32_t seed, uint32_t iter, long long lane) {
   if (eps != nullptr) {
@@ -236,6 +238,25 @@ __device__ __forceinline__ void draw_eps(float (&e)[A], const float* __restrict_
     noise4<(A + 1) / 2>(B200RL_NOISE_NORMAL, seed, iter, 0, lane, row, 0, q);
 #pragma unroll
     for (int a = 0; a < A; ++a) e[a] = q[a];
+  }
+}
+
+// A > 4: chunk c of the Philox stream holds eps[4c .. 4c+3], as in draw_reset and b200rl_fill_noise.
+template <int A, typename std::enable_if<(A > 4), int>::type = 0>
+__device__ __forceinline__ void draw_eps(float (&e)[A], const float* __restrict__ eps, int row, long long N,
+                                         long long n, uint32_t seed, uint32_t iter, long long lane) {
+  if (eps != nullptr) {
+#pragma unroll
+    for (int a = 0; a < A; ++a) e[a] = eps[((size_t)row * A + a) * N + n];
+  } else {
+#pragma unroll
+    for (int c = 0; c < (A + 3) / 4; ++c) {
+      float q[4];
+      noise4<2>(B200RL_NOISE_NORMAL, seed, iter, 0, lane, row, c, q);   // an unused last pair is dead code
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+        if (c * 4 + i < A) e[c * 4 + i] = q[i];
+    }
   }
 }
 

@@ -161,6 +161,7 @@ __device__ __forceinline__ float clamp_log_std(float param, float log_min_std) {
   B200RL_DISPATCH_NET_OA(6, 1, H_, __VA_ARGS__)                                              \
   B200RL_DISPATCH_NET_OA(13, 2, H_, __VA_ARGS__)                                             \
   B200RL_DISPATCH_NET_OA(20, 3, H_, __VA_ARGS__)                                             \
+  B200RL_DISPATCH_NET_OA(20, 6, H_, __VA_ARGS__)                                             \
   {                                                                                          \
     ::b200rl::set_error("network shape O=%d A=%d hidden=(%d,%d) is not compiled in", obs_dim, act_dim, h1, h2); \
     return B200RL_EUNSUPPORTED;                                                              \
@@ -179,6 +180,8 @@ __device__ __forceinline__ float clamp_log_std(float param, float log_min_std) {
   B200RL_DISPATCH_NET_OA(6, 1, 64, __VA_ARGS__)                                              \
   B200RL_DISPATCH_NET_OA(13, 2, 64, __VA_ARGS__)                                             \
   B200RL_DISPATCH_NET_OA(20, 3, 64, __VA_ARGS__)                                             \
+  B200RL_DISPATCH_NET_OA(20, 6, 32, __VA_ARGS__)                                             \
+  B200RL_DISPATCH_NET_OA(20, 6, 64, __VA_ARGS__)                                             \
   {                                                                                          \
     ::b200rl::set_error("network shape O=%d A=%d hidden=(%d,%d) is not compiled in", obs_dim, act_dim, h1, h2); \
     return B200RL_EUNSUPPORTED;                                                              \
@@ -186,7 +189,8 @@ __device__ __forceinline__ float clamp_log_std(float param, float log_min_std) {
 
 inline bool net_supported(int O, int h1, int h2, int A) {
   if (h1 != h2 || (h1 != 32 && h1 != 64)) return false;
-  return (O == 2 && A == 2) || (O == 4 && A == 1) || (O == 3 && A == 1) || (O == 6 && A == 1) || (O == 13 && A == 2) || (O == 20 && A == 3);
+  return (O == 2 && A == 2) || (O == 4 && A == 1) || (O == 3 && A == 1) || (O == 6 && A == 1) || (O == 13 && A == 2) || (O == 20 && A == 3) ||
+         (O == 20 && A == 6);
 }
 
 }  // namespace b200rl

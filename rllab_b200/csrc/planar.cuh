@@ -1,13 +1,14 @@
-// Planar articulated-body environments: rllab's MuJoCo Swimmer and Hopper restated as planar serial chains
-// (generalised coordinates, M(q) qacc + bias = tau, semi-implicit Euler x50 / RK4, inertia-box fluid forces, soft
-// joint-limit and contact constraints solved by a fixed number of projected Gauss-Seidel sweeps).
-// One thread per lane, everything in registers, float32.  The float64 statement of the same model is
-// oracle/planar.py (which documents the modelling choices and cites the reference files); the two must agree to
-// float32 tolerance (tests/test_gpu_kernels.py::test_env_step_matches_oracle).
+// Planar articulated-body environments: rllab's MuJoCo Swimmer, Hopper and HalfCheetah restated as planar kinematic
+// trees (generalised coordinates, M(q) qacc + bias = tau, semi-implicit Euler x50 / RK4 / Euler, inertia-box fluid
+// forces, soft joint-limit and contact constraints solved by a fixed number of projected Gauss-Seidel sweeps).
+// One thread per lane, float32, everything in registers except HalfCheetah's active constraint rows (local memory).
+// The float64 statement of the same models is oracle/planar.py (serial chains) and tests/planar_tree_oracle.py (the
+// tree, HalfCheetah), which document the modelling choices and cite the reference files; they must agree to float32
+// tolerance (tests/test_gpu_kernels.py::test_env_step_matches_oracle, tests/test_gpu_half_cheetah.py).
 //
 // Reference call sites: rllab/envs/mujoco/mujoco_env.py:109-132,184-191, swimmer_env.py:25-45, hopper_env.py:38-61,
-// rllab/mujoco_py/mjcore.py:58-81, vendor/mujoco_models/{swimmer,hopper}.xml.  The arithmetic of the closed
-// MuJoCo 1.31 binary is absent: PARITY UNPINNED (SURVEY.md 8c).
+// half_cheetah_env.py:22-48, rllab/mujoco_py/mjcore.py:58-81, vendor/mujoco_models/{swimmer,hopper,half_cheetah}.xml.
+// The arithmetic of the closed MuJoCo 1.31 binary is absent: PARITY UNPINNED (SURVEY.md 8c).
 #pragma once
 #define B200RL_HAVE_PLANAR 1
 #include "common.cuh"
@@ -28,12 +29,39 @@ __host__ __device__ constexpr CapsuleC capsule_c(double r, double L) {
                   (float)(mc * r * r / 2 + 2 * mh * (2 * r * r / 5))};
 }
 
+// Defaults of the model terms that only HalfCheetah uses; each leaves the Swimmer / Hopper arithmetic unchanged.
+struct PlanarModelDefaults {
+  static constexpr float y0 = 0.f;                      // world height of the root body at rootz = 0
+  static constexpr bool active_rows = false;            // PGS over the compacted active rows (else dense, in registers)
+  // joint limits: solref (.02, 1), solimp (.9, .95, .001);  contacts: solref (.02, 1), solimp (.8, .8, .01)
+  static constexpr float lim_tc = 0.02f, lim_d0 = 0.9f, lim_d1 = 0.95f, lim_w = 0.001f;
+  static constexpr float con_tc = 0.02f, con_d0 = 0.8f, con_d1 = 0.8f, con_w = 0.01f;
+  __host__ __device__ static constexpr float stiffness(int) { return 0.f; }   // spring to qpos0 = 0
+  __host__ __device__ static constexpr float gear(int) { return 1.f; }
+};
+
+// Topology: body i hangs from M::parent(i) < i (body 0 is the root); M::is_ancestor(k, i): k is an ancestor of i, or i
+// itself, stated in closed form so that it folds inside the unrolled Jacobian loops.  planar_topology_ok checks the two
+// against each other at compile time.
+template <class M>
+__host__ __device__ constexpr bool planar_topology_ok() {
+  for (int i = 0; i < M::n; ++i)
+    for (int k = 0; k < M::n; ++k) {
+      int j = i;
+      while (j > k) j = M::parent(j);
+      if (M::is_ancestor(k, i) != (j == k) || (i > 0 && M::parent(i) >= i)) return false;
+    }
+  return true;
+}
+
 // ---------------------------------------------------------------- model descriptions (compile-time accessors)
-struct SwimmerModel {
+struct SwimmerModel : PlanarModelDefaults {
   static constexpr int n = 3, nv = 5, nu = 2, iX = 0, iY = 1, nlim = 2, ncon = 0;
   static constexpr bool rk4 = false, fluid = true;
   static constexpr int frame_skip = 50;
   static constexpr float dt = 0.001f, gX = 0.f, gY = 0.f, density = 4000.f, viscosity = 0.1f, ctrl_lim = 50.f;
+  __host__ __device__ static constexpr int parent(int i) { return i - 1; }
+  __host__ __device__ static constexpr bool is_ancestor(int k, int i) { return k <= i; }
   __host__ __device__ static constexpr float sgn(int) { return 1.f; }
   __host__ __device__ static constexpr float ax(int i) { return i == 1 ? 0.5f : (i == 2 ? -1.f : 0.f); }
   __host__ __device__ static constexpr float ay(int) { return 0.f; }
@@ -59,11 +87,13 @@ struct SwimmerModel {
   static constexpr float mu = 0.f, margin = 0.f;
 };
 
-struct HopperModel {
+struct HopperModel : PlanarModelDefaults {
   static constexpr int n = 4, nv = 6, nu = 3, iX = 1, iY = 0, nlim = 3, ncon = 2;
   static constexpr bool rk4 = true, fluid = false;
   static constexpr int frame_skip = 1;
   static constexpr float dt = 0.02f, gX = 0.f, gY = -9.81f, density = 0.f, viscosity = 0.f, ctrl_lim = 200.f;
+  __host__ __device__ static constexpr int parent(int i) { return i - 1; }
+  __host__ __device__ static constexpr bool is_ancestor(int k, int i) { return k <= i; }
   __host__ __device__ static constexpr float sgn(int i) { return i == 0 ? -1.f : 1.f; }
   __host__ __device__ static constexpr float ax(int) { return 0.f; }
   __host__ __device__ static constexpr float ay(int i) { return i == 1 ? -0.2f : (i == 2 ? -0.45f : (i == 3 ? -0.5f : 0.f)); }
@@ -90,6 +120,128 @@ struct HopperModel {
   static constexpr float mu = 2.0f, margin = 0.001f;
 };
 
+// vendor/mujoco_models/half_cheetah.xml.  Bodies: 0 torso, 1 bthigh, 2 bshin, 3 bfoot, 4 fthigh, 5 fshin, 6 ffoot;
+// q = [rootx, rootz, rooty, bthigh, bshin, bfoot, fthigh, fshin, ffoot] (plane X = x, Y = z, every hinge about +y).
+// Eight capsules of radius .046 (the torso body carries `torso` and `head`); body masses and inertias are summed over a
+// body's capsules with the parallel-axis theorem, then scaled by settotalmass = 14 / (total geom mass).
+struct CheetahGeom {
+  int body;
+  double hl, px, py;   // capsule half-length and centre (body frame, (x, z)); its axis lies in the plane, so Iyy = Ip
+};
+__host__ __device__ constexpr CheetahGeom cheetah_geom(int g) {
+  return g == 0 ? CheetahGeom{0, 0.5, 0.0, 0.0} : g == 1 ? CheetahGeom{0, 0.15, 0.6, 0.1}
+       : g == 2 ? CheetahGeom{1, 0.145, 0.1, -0.13} : g == 3 ? CheetahGeom{2, 0.15, -0.14, -0.07}
+       : g == 4 ? CheetahGeom{3, 0.094, 0.03, -0.097} : g == 5 ? CheetahGeom{4, 0.133, -0.07, -0.12}
+       : g == 6 ? CheetahGeom{5, 0.106, 0.065, -0.09} : CheetahGeom{6, 0.07, 0.045, -0.07};
+}
+constexpr double CHEETAH_R = 0.046;
+__host__ __device__ constexpr double cheetah_geom_m(int g) {
+  const double r = CHEETAH_R, L = 2 * cheetah_geom(g).hl, pi = 3.14159265358979323846;
+  return 1000.0 * pi * r * r * L + 2 * 1000.0 * (2.0 / 3.0) * pi * r * r * r;
+}
+__host__ __device__ constexpr double cheetah_geom_Ip(int g) {
+  const double r = CHEETAH_R, L = 2 * cheetah_geom(g).hl, pi = 3.14159265358979323846;
+  const double mc = 1000.0 * pi * r * r * L, mh = 1000.0 * (2.0 / 3.0) * pi * r * r * r;
+  return mc * (r * r / 4 + L * L / 12) + 2 * mh * (2 * r * r / 5 + L * L / 4 + 3 * L * r / 8);
+}
+__host__ __device__ constexpr double cheetah_mass_scale() {
+  double s = 0.0;
+  for (int g = 0; g < 8; ++g) s += cheetah_geom_m(g);
+  return 14.0 / s;
+}
+// unscaled body mass, COM (axis 0: x, 1: z) and inertia about the COM
+__host__ __device__ constexpr double cheetah_body_m(int b) {
+  double m = 0.0;
+  for (int g = 0; g < 8; ++g) m += cheetah_geom(g).body == b ? cheetah_geom_m(g) : 0.0;
+  return m;
+}
+__host__ __device__ constexpr double cheetah_body_c(int b, int axis) {
+  double s = 0.0;
+  for (int g = 0; g < 8; ++g)
+    s += cheetah_geom(g).body == b ? cheetah_geom_m(g) * (axis == 0 ? cheetah_geom(g).px : cheetah_geom(g).py) : 0.0;
+  return s / cheetah_body_m(b);
+}
+__host__ __device__ constexpr double cheetah_body_I(int b) {
+  double s = 0.0;
+  for (int g = 0; g < 8; ++g) {
+    if (cheetah_geom(g).body != b) continue;
+    const double dx = cheetah_geom(g).px - cheetah_body_c(b, 0), dy = cheetah_geom(g).py - cheetah_body_c(b, 1);
+    s += cheetah_geom_Ip(g) + cheetah_geom_m(g) * (dx * dx + dy * dy);
+  }
+  return s;
+}
+
+struct HalfCheetahModel : PlanarModelDefaults {
+  static constexpr int n = 7, nv = 9, nu = 6, iX = 0, iY = 1, nlim = 6, ncon = 16;
+  static constexpr bool rk4 = false, fluid = false, active_rows = true;
+  static constexpr int frame_skip = 1;
+  static constexpr float dt = 0.01f, gX = 0.f, gY = -9.81f, density = 0.f, viscosity = 0.f, ctrl_lim = 1.f;
+  static constexpr float y0 = 0.7f;
+  // limits: solreflimit (.02, 1), solimplimit (0, .8, .03);  geoms: solref (.02, 1), solimp (0, .8, .01)
+  static constexpr float lim_tc = 0.02f, lim_d0 = 0.f, lim_d1 = 0.8f, lim_w = 0.03f;
+  static constexpr float con_tc = 0.02f, con_d0 = 0.f, con_d1 = 0.8f, con_w = 0.01f;
+  __host__ __device__ static constexpr int parent(int i) { return (i == 1 || i == 4) ? 0 : i - 1; }
+  __host__ __device__ static constexpr bool is_ancestor(int k, int i) {   // torso -> back leg 1..3, front leg 4..6
+    return k == i || k == 0 || (k <= i && (k >= 4) == (i >= 4));
+  }
+  __host__ __device__ static constexpr float sgn(int) { return -1.f; }
+  __host__ __device__ static constexpr float ax(int i) {
+    return i == 1 ? -0.5f : i == 2 ? 0.16f : i == 3 ? -0.28f : i == 4 ? 0.5f : i == 5 ? -0.14f : i == 6 ? 0.13f : 0.f;
+  }
+  __host__ __device__ static constexpr float ay(int i) {
+    return i == 2 ? -0.25f : i == 3 ? -0.14f : i == 5 ? -0.24f : i == 6 ? -0.18f : 0.f;
+  }
+  __host__ __device__ static constexpr float cx(int i) { return (float)cheetah_body_c(i, 0); }
+  __host__ __device__ static constexpr float cy(int i) { return (float)cheetah_body_c(i, 1); }
+  __host__ __device__ static constexpr float box(int) { return 0.f; }   // every joint sits at its body's origin
+  __host__ __device__ static constexpr float boy(int) { return 0.f; }
+  __host__ __device__ static constexpr CapsuleC cap(int i) {
+    return CapsuleC{(float)(cheetah_mass_scale() * cheetah_body_m(i)), (float)(cheetah_mass_scale() * cheetah_body_I(i)),
+                    0.f};
+  }
+  __host__ __device__ static constexpr float lax(int) { return 0.f; }
+  __host__ __device__ static constexpr float lay(int) { return 0.f; }
+  __host__ __device__ static constexpr float armature(int k) { return k >= 3 ? 0.1f : 0.f; }
+  __host__ __device__ static constexpr float damping(int k) {
+    return k == 3 ? 6.f : k == 4 ? 4.5f : k == 5 ? 3.f : k == 6 ? 4.5f : k == 7 ? 3.f : k == 8 ? 1.5f : 0.f;
+  }
+  __host__ __device__ static constexpr float stiffness(int k) {
+    return k == 3 ? 240.f : k == 4 ? 180.f : k == 5 ? 120.f : k == 6 ? 180.f : k == 7 ? 120.f : k == 8 ? 60.f : 0.f;
+  }
+  __host__ __device__ static constexpr float gear(int j) {
+    return j == 0 ? 120.f : j == 1 ? 90.f : j == 2 ? 60.f : j == 3 ? 120.f : j == 4 ? 60.f : 30.f;
+  }
+  __host__ __device__ static constexpr int act(int j) { return j + 1; }
+  __host__ __device__ static constexpr int lim_hinge(int j) { return j + 1; }
+  __host__ __device__ static constexpr float lim_lo(int j) {
+    return j == 0 ? -0.52f : j == 1 ? -0.785f : j == 2 ? -0.4f : j == 3 ? -1.f : j == 4 ? -1.2f : -0.5f;
+  }
+  __host__ __device__ static constexpr float lim_hi(int j) {
+    return j == 0 ? 1.05f : j == 1 ? 0.785f : j == 2 ? 0.785f : j == 3 ? 0.7f : j == 4 ? 0.87f : 0.5f;
+  }
+  __host__ __device__ static constexpr float q0(int) { return 0.f; }
+  // contact candidates: both end spheres of every capsule, centre +- hl (sin a, cos a) for axisangle (0 1 0 a), in geom
+  // order (torso, head, bthigh, bshin, bfoot, fthigh, fshin, ffoot), minus end first
+  __host__ __device__ static constexpr int con_body(int c) { return cheetah_geom(c / 2).body; }
+  __host__ __device__ static constexpr float con_ex(int c) {
+    constexpr float e[16] = {-0.5f, 0.5f, 0.48535067f, 0.7146493f, 0.011280606f, 0.18871939f, -0.005539139f,
+                             -0.27446085f, 0.055072755f, 0.004927245f, -0.13608506f, -0.0039149416f, 0.1248521f,
+                             0.0051478976f, 0.084524974f, 0.005475027f};
+    return e[c];
+  }
+  __host__ __device__ static constexpr float con_ey(int c) {
+    constexpr float e[16] = {0.f, 0.f, 0.003276018f, 0.19672398f, -0.015309682f, -0.24469031f, -0.0035148377f,
+                             -0.13648516f, -0.18759446f, -0.0064055356f, -0.23541994f, -0.0045800493f, -0.17748557f,
+                             -0.0025144247f, -0.1277735f, -0.012226507f};
+    return e[c];
+  }
+  __host__ __device__ static constexpr float con_r(int) { return 0.046f; }
+  static constexpr float mu = 0.4f, margin = 0.f;
+};
+
+static_assert(planar_topology_ok<SwimmerModel>() && planar_topology_ok<HopperModel>() &&
+              planar_topology_ok<HalfCheetahModel>(), "is_ancestor must match parent");
+
 struct PlanarKin {
   float comX, comY, comvelX;
 };
@@ -104,9 +256,141 @@ __device__ __forceinline__ void planar_sincos(float x, float* s, float* c) {
   __sincosf(r, s, c);
 }
 
-// d(r) = d0 + (d1-d0) min(|r|/width, 1)
+// d(r) = d0 + (d1-d0) min(|r|/width, 1), clamped to MuJoCo's [1e-4, 0.9999] when d0 or d1 lies outside it (d0 = 0 would
+// make R = (1-d)/d A infinite at r = 0).  d0, d1 are compile-time constants, so the test folds away.
 __device__ __forceinline__ float planar_imp(float d0, float d1, float w, float r) {
-  return d0 + (d1 - d0) * fminf(fabsf(r) * (1.0f / w), 1.0f);
+  const float d = d0 + (d1 - d0) * fminf(fabsf(r) * (1.0f / w), 1.0f);
+  return (fminf(d0, d1) < 1e-4f || fmaxf(d0, d1) > 0.9999f) ? fminf(fmaxf(d, 1e-4f), 0.9999f) : d;
+}
+
+// Body angles, angular velocities and their sin / cos down the tree: phi_i = phi_parent(i) + s_i q_hinge_i.
+template <class M>
+__device__ __forceinline__ void planar_angles(const float (&q)[M::nv], const float (&v)[M::nv], float (&om)[M::n],
+                                              float (&cs)[M::n], float (&sn)[M::n]) {
+  float ap[M::n];
+#pragma unroll
+  for (int i = 0; i < M::n; ++i) {
+    ap[i] = (i == 0 ? 0.f : ap[M::parent(i)]) + M::sgn(i) * q[2 + i];
+    om[i] = (i == 0 ? 0.f : om[M::parent(i)]) + M::sgn(i) * v[2 + i];
+    planar_sincos(ap[i], &sn[i], &cs[i]);
+  }
+}
+
+// Constraint solve over the active rows only (models with active_rows): HalfCheetah has 6 limit + 32 contact rows, and
+// the dense (A + R) system of planar_dynamics does not fit in registers.  Active rows are compacted, in the all-rows
+// order, into local-memory arrays sized for every row (nothing is dropped), and PGS runs matrix-free on them:
+// sum_j A_ij f_j = J_i . w with w = M^-1 J^T f kept up to date after each row.  Inactive rows have f = 0 in the all-rows
+// statement, so this is the same system and the same sweep order.
+template <class M, class Solve>
+__device__ __forceinline__ void planar_constraints_active(const float (&q)[M::nv], const float (&v)[M::nv],
+                                                          const float (&cs)[M::n], const float (&sn)[M::n],
+                                                          const float (&hx)[M::n], const float (&hy)[M::n],
+                                                          const float (&tau)[M::nv], const float (&a0)[M::nv],
+                                                          Solve& solve, float (&acc)[M::nv], float (&qfc)[M::nv]) {
+  constexpr int nv = M::nv, NC = M::nlim + 2 * M::ncon;
+  float cJ[NC][nv], cMiJ[NC][nv], crhs[NC], cR[NC], cid[NC], cf[NC];
+  int cnrm[NC];   // -1: unilateral row (limit, contact normal); else the slot of the tangential row's normal
+  int m = 0;
+  auto push = [&](const float (&J)[nv], float aref, float d, int nrm) {
+    float MiJ[nv];
+    solve(J, MiJ);
+    float Aii = 0.f, Ja0 = 0.f;
+#pragma unroll
+    for (int k = 0; k < nv; ++k) { Ja0 += J[k] * a0[k]; Aii += J[k] * MiJ[k]; }
+#pragma unroll
+    for (int k = 0; k < nv; ++k) { cJ[m][k] = J[k]; cMiJ[m][k] = MiJ[k]; }
+    crhs[m] = aref - Ja0;
+    cR[m] = (1.0f - d) / d * Aii;
+    cid[m] = 1.0f / (Aii + cR[m]);
+    cf[m] = 0.f;
+    cnrm[m] = nrm;
+    ++m;
+  };
+  {
+    const float dmax = fmaxf(M::lim_d0, M::lim_d1), tc = M::lim_tc;
+    const float bb = 2.0f / (dmax * tc), kk = 1.0f / (dmax * dmax * tc * tc);
+#pragma unroll
+    for (int j = 0; j < M::nlim; ++j) {
+      const int hk = 2 + M::lim_hinge(j);
+      const float rlo = q[hk] - M::lim_lo(j), rhi = M::lim_hi(j) - q[hk];
+      const bool hi = rhi < 0.f;
+      if (!(rlo < 0.f || hi)) continue;
+      const float sg = hi ? -1.f : 1.f, r_ = hi ? rhi : rlo;
+      float J[nv];
+#pragma unroll
+      for (int k = 0; k < nv; ++k) J[k] = 0.f;
+      J[hk] = sg;
+      const float d = planar_imp(M::lim_d0, M::lim_d1, M::lim_w, r_);
+      push(J, -bb * (sg * v[hk]) - kk * d * r_, d, -1);
+    }
+  }
+  {
+    const float dmax = fmaxf(M::con_d0, M::con_d1), tc = M::con_tc;
+    const float bb = 2.0f / (dmax * tc), kk = 1.0f / (dmax * dmax * tc * tc);
+#pragma unroll
+    for (int c = 0; c < M::ncon; ++c) {
+      const int bi = M::con_body(c);
+      const float ex = cs[bi] * M::con_ex(c) - sn[bi] * M::con_ey(c), ey = sn[bi] * M::con_ex(c) + cs[bi] * M::con_ey(c);
+      const float sx = hx[bi] + ex, sy = hy[bi] + ey;
+      const float r_ = sy - M::con_r(c) - M::margin;
+      if (!(r_ < 0.f)) continue;
+      const float ptx = sx, pty = sy - M::con_r(c);
+      float Jn[nv], Jt[nv];
+#pragma unroll
+      for (int k = 0; k < nv; ++k) { Jn[k] = 0.f; Jt[k] = 0.f; }
+      Jt[M::iX] = 1.f; Jn[M::iY] = 1.f;
+#pragma unroll
+      for (int k = 0; k <= bi; ++k) {
+        if (!M::is_ancestor(k, bi)) continue;
+        Jt[2 + k] = -M::sgn(k) * (pty - hy[k]);
+        Jn[2 + k] = M::sgn(k) * (ptx - hx[k]);
+      }
+      const float d = planar_imp(M::con_d0, M::con_d1, M::con_w, r_);
+      float vn = 0.f, vt = 0.f;
+#pragma unroll
+      for (int k = 0; k < nv; ++k) { vn += Jn[k] * v[k]; vt += Jt[k] * v[k]; }
+      push(Jn, -bb * vn - kk * d * r_, d, -1);
+      push(Jt, -bb * vt, d, m - 1);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < nv; ++k) qfc[k] = 0.f;
+  if (m == 0) {
+#pragma unroll
+    for (int k = 0; k < nv; ++k) acc[k] = a0[k];
+    return;
+  }
+  float w[nv];
+#pragma unroll
+  for (int k = 0; k < nv; ++k) w[k] = 0.f;
+#pragma unroll 1
+  for (int sweep = 0; sweep < PLANAR_PGS_SWEEPS; ++sweep) {
+#pragma unroll 1
+    for (int i = 0; i < m; ++i) {
+      float s = crhs[i] - cR[i] * cf[i];
+#pragma unroll
+      for (int k = 0; k < nv; ++k) s -= cJ[i][k] * w[k];
+      float fi = cf[i] + s * cid[i];
+      if (cnrm[i] < 0) fi = fmaxf(fi, 0.f);
+      else {
+        const float lim = M::mu * cf[cnrm[i]];
+        fi = fminf(fmaxf(fi, -lim), lim);
+      }
+      const float df = fi - cf[i];
+#pragma unroll
+      for (int k = 0; k < nv; ++k) w[k] = fmaf(cMiJ[i][k], df, w[k]);
+      cf[i] = fi;
+    }
+  }
+  float tot[nv];
+#pragma unroll 1
+  for (int i = 0; i < m; ++i) {
+#pragma unroll
+    for (int k = 0; k < nv; ++k) qfc[k] += cJ[i][k] * cf[i];
+  }
+#pragma unroll
+  for (int k = 0; k < nv; ++k) tot[k] = tau[k] + qfc[k];
+  solve(tot, acc);
 }
 
 // qacc, qfrc_constraint and COM quantities at (q, v, ctrl).
@@ -116,25 +400,18 @@ __device__ __forceinline__ void planar_dynamics(const float (&q)[M::nv], const f
   constexpr int n = M::n, nv = M::nv;
   // ---- kinematics
   float om[n], cs[n], sn[n];
-  {
-    float ap = 0.f, aw = 0.f;
-#pragma unroll
-    for (int i = 0; i < n; ++i) {
-      ap += M::sgn(i) * q[2 + i];
-      aw += M::sgn(i) * v[2 + i];
-      om[i] = aw;
-      planar_sincos(ap, &sn[i], &cs[i]);
-    }
-  }
+  planar_angles<M>(q, v, om, cs, sn);
   float hx[n], hy[n], hdx[n], hdy[n], hddx[n], hddy[n];
-  hx[0] = q[M::iX]; hy[0] = q[M::iY]; hdx[0] = v[M::iX]; hdy[0] = v[M::iY]; hddx[0] = 0.f; hddy[0] = 0.f;
+  hx[0] = q[M::iX]; hy[0] = M::y0 == 0.f ? q[M::iY] : q[M::iY] + M::y0;
+  hdx[0] = v[M::iX]; hdy[0] = v[M::iY]; hddx[0] = 0.f; hddy[0] = 0.f;
 #pragma unroll
   for (int i = 1; i < n; ++i) {
-    const float rax = cs[i - 1] * M::ax(i) - sn[i - 1] * M::ay(i), ray = sn[i - 1] * M::ax(i) + cs[i - 1] * M::ay(i);
-    hx[i] = hx[i - 1] + rax; hy[i] = hy[i - 1] + ray;
-    hdx[i] = hdx[i - 1] - om[i - 1] * ray; hdy[i] = hdy[i - 1] + om[i - 1] * rax;
-    const float w2 = om[i - 1] * om[i - 1];
-    hddx[i] = hddx[i - 1] - w2 * rax; hddy[i] = hddy[i - 1] - w2 * ray;
+    const int p = M::parent(i);
+    const float rax = cs[p] * M::ax(i) - sn[p] * M::ay(i), ray = sn[p] * M::ax(i) + cs[p] * M::ay(i);
+    hx[i] = hx[p] + rax; hy[i] = hy[p] + ray;
+    hdx[i] = hdx[p] - om[p] * ray; hdy[i] = hdy[p] + om[p] * rax;
+    const float w2 = om[p] * om[p];
+    hddx[i] = hddx[p] - w2 * rax; hddy[i] = hddy[p] - w2 * ray;
   }
   // ---- mass matrix (upper), generalised forces
   float Mm[nv][nv], tau[nv];
@@ -158,7 +435,8 @@ __device__ __forceinline__ void planar_dynamics(const float (&q)[M::nv], const f
     for (int k = 0; k < nv; ++k) { JX[k] = 0.f; JY[k] = 0.f; wv[k] = 0.f; }
     JX[M::iX] = 1.f; JY[M::iY] = 1.f;
 #pragma unroll
-    for (int k = 0; k <= i; ++k) {
+    for (int k = 0; k <= i; ++k) {   // ancestors precede their descendants
+      if (!M::is_ancestor(k, i)) continue;
       JX[2 + k] = -M::sgn(k) * (py - hy[k]);
       JY[2 + k] = M::sgn(k) * (px - hx[k]);
       wv[2 + k] = M::sgn(k);
@@ -194,9 +472,10 @@ __device__ __forceinline__ void planar_dynamics(const float (&q)[M::nv], const f
   for (int r = 0; r < nv; ++r) {
     Mm[r][r] += M::armature(r);
     tau[r] -= M::damping(r) * v[r];
+    if (M::stiffness(r) != 0.f) tau[r] -= M::stiffness(r) * q[r];
   }
 #pragma unroll
-  for (int j = 0; j < M::nu; ++j) tau[2 + M::act(j)] += fminf(fmaxf(ctrl[j], -M::ctrl_lim), M::ctrl_lim);
+  for (int j = 0; j < M::nu; ++j) tau[2 + M::act(j)] += M::gear(j) * fminf(fmaxf(ctrl[j], -M::ctrl_lim), M::ctrl_lim);
   // ---- Cholesky (lower factor stored in the lower triangle of Mm)
   float idg[nv];
 #pragma unroll
@@ -235,12 +514,16 @@ __device__ __forceinline__ void planar_dynamics(const float (&q)[M::nv], const f
   for (int k = 0; k < nv; ++k) qfc[k] = 0.f;
 
   // ---- constraints
+  if constexpr (M::active_rows) {
+    planar_constraints_active<M>(q, v, cs, sn, hx, hy, tau, a0, solve, acc, qfc);
+    return;
+  }
   constexpr int NC = M::nlim + 2 * M::ncon;
   float J[NC][nv], aref[NC], dimp[NC];
   bool active[NC];
   bool any = false;
   {
-    const float dmax = 0.95f, tc = 0.02f;                    // joint limits: solref (.02,1), solimp (.9,.95,.001)
+    const float dmax = fmaxf(M::lim_d0, M::lim_d1), tc = M::lim_tc;
     const float bb = 2.0f / (dmax * tc), kk = 1.0f / (dmax * dmax * tc * tc);
 #pragma unroll
     for (int j = 0; j < M::nlim; ++j) {
@@ -252,14 +535,14 @@ __device__ __forceinline__ void planar_dynamics(const float (&q)[M::nv], const f
 #pragma unroll
       for (int k = 0; k < nv; ++k) J[j][k] = 0.f;
       J[j][hk] = sg;
-      dimp[j] = planar_imp(0.9f, 0.95f, 0.001f, r_);
+      dimp[j] = planar_imp(M::lim_d0, M::lim_d1, M::lim_w, r_);
       aref[j] = -bb * (sg * v[hk]) - kk * dimp[j] * r_;
       active[j] = lo || hi;
       any = any || active[j];
     }
   }
   if (M::ncon > 0) {
-    const float dmax = 0.8f, tc = 0.02f;                     // geoms: solref (.02,1), solimp (.8,.8,.01)
+    const float dmax = fmaxf(M::con_d0, M::con_d1), tc = M::con_tc;
     const float bb = 2.0f / (dmax * tc), kk = 1.0f / (dmax * dmax * tc * tc);
 #pragma unroll
     for (int c = 0; c < M::ncon; ++c) {
@@ -274,11 +557,12 @@ __device__ __forceinline__ void planar_dynamics(const float (&q)[M::nv], const f
       J[rt][M::iX] = 1.f; J[rn][M::iY] = 1.f;
 #pragma unroll
       for (int k = 0; k <= bi; ++k) {
+        if (!M::is_ancestor(k, bi)) continue;
         J[rt][2 + k] = -M::sgn(k) * (pty - hy[k]);
         J[rn][2 + k] = M::sgn(k) * (ptx - hx[k]);
       }
       const float r_ = dist - M::margin;
-      const float d = planar_imp(0.8f, 0.8f, 0.01f, r_);
+      const float d = planar_imp(M::con_d0, M::con_d1, M::con_w, r_);
       float vn = 0.f, vt = 0.f;
 #pragma unroll
       for (int k = 0; k < nv; ++k) { vn += J[rn][k] * v[k]; vt += J[rt][k] * v[k]; }
@@ -347,25 +631,21 @@ template <class M>
 __device__ __forceinline__ void planar_kin(const float (&q)[M::nv], const float (&v)[M::nv], PlanarKin& kin) {
   constexpr int n = M::n;
   float om[n], cs[n], sn[n];
-  {
-    float ap = 0.f, aw = 0.f;
-#pragma unroll
-    for (int i = 0; i < n; ++i) {
-      ap += M::sgn(i) * q[2 + i];
-      aw += M::sgn(i) * v[2 + i];
-      om[i] = aw;
-      planar_sincos(ap, &sn[i], &cs[i]);
-    }
-  }
-  float hx = q[M::iX], hy = q[M::iY], hdx = v[M::iX], hdy = v[M::iY];
+  planar_angles<M>(q, v, om, cs, sn);
+  // (hx, hy, hdx, hdy): hinge of the current body; the arrays keep every hinge for the children of a branching body
+  float hx = q[M::iX], hy = M::y0 == 0.f ? q[M::iY] : q[M::iY] + M::y0, hdx = v[M::iX], hdy = v[M::iY];
+  float hxs[n], hys[n], hdxs[n], hdys[n];
   float mt = 0.f, comX = 0.f, comY = 0.f, cvX = 0.f;
 #pragma unroll
   for (int i = 0; i < n; ++i) {
     if (i > 0) {
-      const float rax = cs[i - 1] * M::ax(i) - sn[i - 1] * M::ay(i), ray = sn[i - 1] * M::ax(i) + cs[i - 1] * M::ay(i);
+      const int p = M::parent(i);
+      if (p != i - 1) { hx = hxs[p]; hy = hys[p]; hdx = hdxs[p]; hdy = hdys[p]; }
+      const float rax = cs[p] * M::ax(i) - sn[p] * M::ay(i), ray = sn[p] * M::ax(i) + cs[p] * M::ay(i);
       hx += rax; hy += ray;
-      hdx -= om[i - 1] * ray; hdy += om[i - 1] * rax;
+      hdx -= om[p] * ray; hdy += om[p] * rax;
     }
+    hxs[i] = hx; hys[i] = hy; hdxs[i] = hdx; hdys[i] = hdy;
     const CapsuleC cp = M::cap(i);
     const float rcx = cs[i] * M::cx(i) - sn[i] * M::cy(i), rcy = sn[i] * M::cx(i) + cs[i] * M::cy(i);
     const float roy = sn[i] * M::box(i) + cs[i] * M::boy(i);
@@ -508,6 +788,46 @@ struct HopperEnvD {
     for (int k = 0; k < 6; ++k) { s[k] = q[k]; s[6 + k] = v[k]; s[15 + k] = qf[k]; }
     s[12] = u[0]; s[13] = u[1]; s[14] = u[2];
     s[21] = kin.comX; s[22] = kin.comY;
+  }
+};
+
+// ---------------------------------------------------------------- rllab/envs/mujoco/half_cheetah_env.py:14-48
+// state = [qpos 9, qvel 9]; obs = [qpos[1:], qvel, torso subtree COM (x, 0, z)] (mujoco_env.py:184-191 leaves mjData at
+// the post-step state, so obs needs positions only); reward = torso subtree "COM velocity" x (body-origin velocities,
+// mjcore.py:58-81) - 0.05 sum clip(a, -1, 1)^2; never done.
+struct HalfCheetahEnvD {
+  using M = HalfCheetahModel;
+  static constexpr int KIND = B200RL_ENV_HALF_CHEETAH, O = 20, A = 6, S = 18, K = 18, NOISE = B200RL_NOISE_NORMAL;
+  __host__ __device__ static constexpr float lb(int) { return -1.0f; }
+  __host__ __device__ static constexpr float ub(int) { return 1.0f; }
+  __device__ static void reset(float (&s)[S], const float (&raw)[K]) {
+#pragma unroll
+    for (int k = 0; k < 9; ++k) { s[k] = M::q0(k) + 0.01f * raw[k]; s[9 + k] = 0.1f * raw[9 + k]; }
+  }
+  __device__ static void obs(const float (&s)[S], float (&o)[O]) {
+    float q[9], v[9];
+    PlanarKin kin;
+#pragma unroll
+    for (int k = 0; k < 9; ++k) { q[k] = s[k]; v[k] = s[9 + k]; }
+    planar_kin<M>(q, v, kin);
+#pragma unroll
+    for (int k = 0; k < 17; ++k) o[k] = s[1 + k];
+    o[17] = kin.comX; o[18] = 0.f; o[19] = kin.comY;
+  }
+  __device__ static void step(float (&s)[S], const float (&u)[A], float& r, bool& done) {
+    float q[9], v[9];
+    PlanarKin kin;
+#pragma unroll
+    for (int k = 0; k < 9; ++k) { q[k] = s[k]; v[k] = s[9 + k]; }
+    planar_integrate<M>(q, v, u);
+    planar_kin<M>(q, v, kin);
+    float cost = 0.f;
+#pragma unroll
+    for (int k = 0; k < A; ++k) { const float c = fminf(fmaxf(u[k], -1.f), 1.f); cost += c * c; }
+    r = kin.comvelX - 0.05f * cost;
+#pragma unroll
+    for (int k = 0; k < 9; ++k) { s[k] = q[k]; s[9 + k] = v[k]; }
+    done = false;
   }
 };
 

@@ -33,11 +33,12 @@ constexpr int POP_STREAM = 2;              // Philox stream of the parameter dra
 template <class Env, int H>
 constexpr int pop_minblocks() { return (H == 32 && Env::S <= 4) ? 4 : 1; }
 
-// Per-warp shared memory, in floats: activation row [H], Wout [H][A], bout [4], and W1 [H][H] for 64-wide nets and for
-// Hopper (its 23-float state and 20 inputs leave no room for a register-resident W1 column).
+// Per-warp shared memory, in floats: activation row [H], Wout [H][A], bout [A rounded up to 4], and W1 [H][H] for
+// 64-wide nets and for 20-input nets (Hopper's 23-float state and HalfCheetah's 18 leave no room for a
+// register-resident W1 column).
 template <class Env, int H>
 struct PopLayout {
-  static constexpr int oH = 0, oWo = oH + H, oBo = oWo + H * Env::A, oW1 = oBo + 4;
+  static constexpr int oH = 0, oWo = oH + H, oBo = oWo + H * Env::A, oW1 = oBo + ((Env::A + 3) & ~3);
   static constexpr bool W1_SMEM = H > 32 || Env::O > 13;
   static constexpr int FLOATS = oW1 + (W1_SMEM ? H * H : 0);
   static_assert(oWo % 4 == 0 && oBo % 4 == 0 && oW1 % 4 == 0, "float4 alignment of the per-warp rows");

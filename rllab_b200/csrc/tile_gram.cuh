@@ -11,15 +11,18 @@
 
 namespace b200rl {
 
-// distribution constants of one pass (A <= 3); FVP: old == new
+// distribution constants of one pass (A <= TILE_AMAX, entries k < A in use; a register-resident local); FVP: old == new
+constexpr int TILE_AMAX = 6;
 struct TileDist {
-  float ls_new[3], inv_std[3], ls_old[3], inv_std_old[3], Mmu[3], var_new[3], var_new2[3], var_old[3];
+  float ls_new[TILE_AMAX], inv_std[TILE_AMAX], ls_old[TILE_AMAX], inv_std_old[TILE_AMAX], Mmu[TILE_AMAX],
+      var_new[TILE_AMAX], var_new2[TILE_AMAX], var_old[TILE_AMAX];
   float sum_ls_new, sum_ls_old, half_log2pi_A;
 };
 
 template <class N, int MODE>
 __device__ __forceinline__ void tile_dist_init(TileDist& D, const float* log_std_params, const UpdArgs& a) {
   constexpr int A = N::A;
+  static_assert(A <= TILE_AMAX, "act_dim beyond the TileDist arrays");
   D.sum_ls_new = 0.f;
   D.sum_ls_old = 0.f;
 #pragma unroll
@@ -43,8 +46,9 @@ __device__ __forceinline__ void tile_dist_init(TileDist& D, const float* log_std
 // RX..RDM: first stage row of X, H1, H2, D1, D2, DM (DL rows follow DM); LD: row pitch in floats (tile + 4).
 // The accumulation is split in two parts so that a caller whose D1 rows only exist later (update_umma32.cu: D1 needs one
 // more tensor-core GEMM) can run part A behind that GEMM, and may alias the D1 rows with the H2 rows (dead after part A):
-//   part A  dW1 = H1^T D2 (all 128 threads: 4x4 register tiles x two K-halves), dWout[:, k] / db1 (warp k / warp 3),
-//           dbout / dlog_std row sums (threads < 2A)                                   -- reads H1, H2, D2, DM, DL
+//   part A  dW1 = H1^T D2 (all 128 threads: 4x4 register tiles x two K-halves), dWout[:, k] / db1 (A <= 3: warp k /
+//           warp 3; A <= 6: job j = column j < A or db1 at j = A, on warp j % 4, slot j / 4), dbout / dlog_std row
+//           sums (threads < 2A)                                                        -- reads H1, H2, D2, DM, DL
 //   part B  dW0[o, :] for o = warp, warp + 4, ... and db0 (warp 3)                     -- reads X, D1
 // Every small output is spread over the four warps: with one warp per output group (the first layout) warp 0 carried
 // dW1 + all of dW0 -- 2.7x the work of the others for obs_dim 13 -- and set the length of the phase.
@@ -53,10 +57,12 @@ template <class N, int RX, int RH1, int RH2, int RD1, int RD2, int RDM, int LD, 
 struct TileGram {
   static constexpr int O = N::O, H = 32, A = N::A, TILE = 128;
   static constexpr int OQ = (O + 3) / 4;          // obs rows per warp in part B
-  static_assert(N::H1 == 32 && N::H2 == 32 && A <= 3, "32-wide layers, act_dim <= 3");
+  static_assert(N::H1 == 32 && N::H2 == 32 && A <= 6, "32-wide layers, act_dim <= 6");
+  static constexpr int NS = A <= 3 ? 1 : 2;       // part-A jobs per warp
+  static constexpr int JDB = A <= 3 ? 3 : A;      // job index of db1
   double accW1[4][4];
   double accB[OQ + 1];   // part B: dW0[warp + 4 i][lane], i < OQ; [OQ]: db0[lane] (warp 3)
-  double accA;           // part A: dWout[lane][warp] (warp < A) | db1[lane] (warp 3)
+  double accA, accA1;    // part A, job j = warp + 4 s (s = 0: accA, 1: accA1): dWout[lane][j] (j < A) | db1 (j == JDB)
   double accT;           // part A: dbout[tid] / dlog_std[tid - A] row sums (tid < 2A)
 
   __device__ __forceinline__ void init() {
@@ -67,6 +73,7 @@ struct TileGram {
 #pragma unroll
     for (int k = 0; k <= OQ; ++k) accB[k] = 0.0;
     accA = 0.0;
+    accA1 = 0.0;
     accT = 0.0;
   }
 
@@ -122,11 +129,15 @@ struct TileGram {
 #pragma unroll
         for (int c = 0; c < 4; ++c) accW1[r][c] += (double)acc[r][c];
     }
-    // small outputs of part A: warp k < A -> dWout[lane][k] = H2[lane] . DM[k]; warp 3 -> db1[lane] = sum D2[lane]
+    // small outputs of part A: job j < A -> dWout[lane][j] = H2[lane] . DM[j]; job JDB -> db1[lane] = sum D2[lane]
     const int lane = tid & 31, wq = tid >> 5;
-    if (wq < A) {
+#pragma unroll
+    for (int s = 0; s < NS; ++s) {
+    const int j = wq + 4 * s;
+    double& acc = s == 0 ? accA : accA1;
+    if (j < A) {
       const float* Hh = stage + (RH2 + lane) * LD;
-      const float* M = stage + (RDM + wq) * LD;
+      const float* M = stage + (RDM + j) * LD;
       float s0 = 0.f, s1 = 0.f;
 #pragma unroll 4
       for (int k = 0; k < TILE; k += 4) {
@@ -135,8 +146,8 @@ struct TileGram {
         s0 = fmaf(hv.x, m.x, s0); s1 = fmaf(hv.y, m.y, s1);
         s0 = fmaf(hv.z, m.z, s0); s1 = fmaf(hv.w, m.w, s1);
       }
-      accA += (double)(s0 + s1);
-    } else if (wq == 3) {
+      acc += (double)(s0 + s1);
+    } else if (j == JDB) {
       const float* Dr = stage + (RD2 + lane) * LD;
       float s0 = 0.f;
 #pragma unroll 4
@@ -144,7 +155,8 @@ struct TileGram {
         const float4 d = *reinterpret_cast<const float4*>(Dr + k);
         s0 += (d.x + d.y) + (d.z + d.w);
       }
-      accA += (double)s0;
+      acc += (double)s0;
+    }
     }
     if (tid < 2 * A) {
       const float* Dr = stage + (RDM + tid) * LD;   // rows DM[0..A-1], DL[0..A-1] are contiguous
@@ -209,11 +221,22 @@ struct TileGram {
       const int o = wq + 4 * i;
       if (o < O) out[N::oW0 + o * H + lane] = accB[i];
     }
-    if (wq == 3) {
-      out[N::ob0 + lane] = accB[OQ];
-      out[N::ob1 + lane] = accA;
-    } else if (wq < A) {
-      out[N::oWo + lane * A + wq] = accA;
+    if constexpr (A <= 3) {
+      if (wq == 3) {
+        out[N::ob0 + lane] = accB[OQ];
+        out[N::ob1 + lane] = accA;
+      } else if (wq < A) {
+        out[N::oWo + lane * A + wq] = accA;
+      }
+    } else {
+      if (wq == 3) out[N::ob0 + lane] = accB[OQ];
+#pragma unroll
+      for (int s = 0; s < NS; ++s) {
+        const int j = wq + 4 * s;
+        const double acc = s == 0 ? accA : accA1;
+        if (j == JDB) out[N::ob1 + lane] = acc;
+        else if (j < A) out[N::oWo + lane * A + j] = acc;
+      }
     }
     if (tid < 2 * A) out[N::obo + tid] = accT;   // obo.. then ols.. are contiguous in the flat layout
   }

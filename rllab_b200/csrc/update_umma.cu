@@ -13,7 +13,7 @@
 //   B   MMA  T1pre = X V0          (K = obs_dim padded to 8)  and, in the same group,  T2pre = H1 V1
 //   C   epilogue: T1 = (T1pre + vb0)(1 - H1^2) -> A operand
 //   D   MMA  T2pre += T1 W1
-//   E   epilogue: T2 = (T2pre + vb1)(1 - H2^2); mu_dot = T2 Wout + H2 Vout + vbout (CUDA cores, N = A <= 3, the four
+//   E   epilogue: T2 = (T2pre + vb1)(1 - H2^2); mu_dot = T2 Wout + H2 Vout + vbout (CUDA cores, N = A <= 6, the four
 //       threads of a row combine by shuffles); dmu = M mu_dot; D2 = (dmu Wout^T)(1 - H2^2) -> A operand + shared-memory rows
 //   F   MMA  D1pre = D2 W1^T, and behind it: dWout / dbout partial sums (warp reduce-scatter of h2[j] dmu[k])
 //   G   epilogue: D1 = D1pre (1 - H1^2) -> shared-memory rows
@@ -55,7 +55,10 @@ struct UmmaSmem {
   static constexpr int o_red = ((o_stage + R * U_LD * 4 + 15) / 16) * 16;     // 3 x 32 doubles: loss / KL block reduction
   static constexpr size_t bytes = (size_t)o_red + 3 * 32 * 8;
   static_assert(bytes <= 232448, "does not fit the 227 KB of shared memory");
-  static_assert(8 * 200 * 4 <= H * U_LD * 4, "the D1 rows must hold the dWout / dbout combine scratch");
+  // dWout / dbout / dlog_std combine scratch, per warp: KG groups of 3 actions x 64 columns, then dbout, dlog_std
+  static constexpr int KG = (A + 2) / 3, SCR = KG == 1 ? 200 : 192 * KG + 16, SBO = 192 * KG, SLS = SBO + (KG == 1 ? 4 : 8);
+  static_assert(A <= 6, "act_dim <= 6");
+  static_assert(8 * SCR * 4 <= H * U_LD * 4, "the D1 rows must hold the dWout / dbout combine scratch");
 };
 
 // element (n, k) of a K-major [64 x K] image, byte offset (k: input feature, stored at u_kperm(k))
@@ -136,8 +139,13 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
 #pragma unroll
   for (int k = 0; k <= OH; ++k) gS[k] = make_float2(0.f, 0.f);
   // dWout: the thread's 16 columns x 3 actions (flat c * 3 + k, c = 2 (column block) + column parity) are reduce-scattered
-  // over the eight row lanes of the warp; lane keeps flat indices wo_base .. wo_base + 5
-  float gWo[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  // over the eight row lanes of the warp; lane keeps flat indices wo_base .. wo_base + 5 (per group g of 3 actions)
+  constexpr int KG = SM::KG;
+  float gWo[KG][6];
+#pragma unroll
+  for (int g = 0; g < KG; ++g)
+#pragma unroll
+    for (int r = 0; r < 6; ++r) gWo[g][r] = 0.f;
   const int wo_base = ((lane >> 4) & 1) * 24 + ((lane >> 3) & 1) * 12 + ((lane >> 2) & 1) * 6;
   float gbo[A], gls[A];               // dbout, dlog_std (GRAD): lane 0 of every warp
 #pragma unroll
@@ -178,36 +186,57 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
 #pragma unroll
     for (int k = 0; k <= OH; ++k) gS[k] = make_float2(0.f, 0.f);
     // dWout / dbout / dlog_std: the eight warps hold partial sums of the same entries -> combine through the (idle) D1
-    // rows in fixed warp order.  scr[warp][200]: [col * 3 + k] dWout, [192 + k] dbout, [196 + k] dlog_std
+    // rows in fixed warp order.  scr[warp][SCR]: [192 g + col * 3 + k] dWout (action 3 g + k), [SBO + k] dbout,
+    // [SLS + k] dlog_std
+    constexpr int SCR = SM::SCR, SBO = SM::SBO, SLS = SM::SLS;
     float* scr = stage + SM::rD1 * LD;
 #pragma unroll
-    for (int r = 0; r < 6; ++r) {
-      const int f = wo_base + r, c = f / 3, k = f % 3;
-      if (k < A) scr[warp * 200 + (8 * (c >> 1) + 2 * t4 + (c & 1)) * 3 + k] = gWo[r];
-    }
+    for (int g = 0; g < KG; ++g)
+#pragma unroll
+      for (int r = 0; r < 6; ++r) {
+        const int f = wo_base + r, c = f / 3, k = f % 3;
+        if (3 * g + k < A) scr[warp * SCR + 192 * g + (8 * (c >> 1) + 2 * t4 + (c & 1)) * 3 + k] = gWo[g][r];
+      }
     if (lane == 0)
 #pragma unroll
       for (int k = 0; k < A; ++k) {
-        scr[warp * 200 + 192 + k] = gbo[k];
-        scr[warp * 200 + 196 + k] = gls[k];
+        scr[warp * SCR + SBO + k] = gbo[k];
+        scr[warp * SCR + SLS + k] = gls[k];
       }
     __syncthreads();
     auto sum8 = [&](int idx) {
-      return ((scr[0 * 200 + idx] + scr[1 * 200 + idx]) + (scr[2 * 200 + idx] + scr[3 * 200 + idx])) +
-             ((scr[4 * 200 + idx] + scr[5 * 200 + idx]) + (scr[6 * 200 + idx] + scr[7 * 200 + idx]));
+      return ((scr[0 * SCR + idx] + scr[1 * SCR + idx]) + (scr[2 * SCR + idx] + scr[3 * SCR + idx])) +
+             ((scr[4 * SCR + idx] + scr[5 * SCR + idx]) + (scr[6 * SCR + idx] + scr[7 * SCR + idx]));
     };
-    if (tid < H * A) {
-      const int col = tid / A, k = tid % A;
-      out[N::oWo + col * A + k] += (double)sum8(col * 3 + k);
-    } else if (tid < H * A + A) {
-      const int k = tid - H * A;
-      out[N::obo + k] += (double)sum8(192 + k);
-    } else if (is_grad_mode(MODE) && tid < H * A + 2 * A) {
-      const int k = tid - H * A - A;
-      out[N::ols + k] += (double)sum8(196 + k);
+    if constexpr (H * A + 2 * A <= U_THREADS) {
+      if (tid < H * A) {
+        const int col = tid / A, k = tid % A;
+        out[N::oWo + col * A + k] += (double)sum8(col * 3 + k);
+      } else if (tid < H * A + A) {
+        const int k = tid - H * A;
+        out[N::obo + k] += (double)sum8(SBO + k);
+      } else if (is_grad_mode(MODE) && tid < H * A + 2 * A) {
+        const int k = tid - H * A - A;
+        out[N::ols + k] += (double)sum8(SLS + k);
+      }
+    } else {
+      for (int e = tid; e < H * A + 2 * A; e += U_THREADS) {
+        if (e < H * A) {
+          const int col = e / A, k = e % A;
+          out[N::oWo + col * A + k] += (double)sum8(192 * (k / 3) + col * 3 + k % 3);
+        } else if (e < H * A + A) {
+          const int k = e - H * A;
+          out[N::obo + k] += (double)sum8(SBO + k);
+        } else if (is_grad_mode(MODE)) {
+          const int k = e - H * A - A;
+          out[N::ols + k] += (double)sum8(SLS + k);
+        }
+      }
     }
 #pragma unroll
-    for (int r = 0; r < 6; ++r) gWo[r] = 0.f;
+    for (int g = 0; g < KG; ++g)
+#pragma unroll
+      for (int r = 0; r < 6; ++r) gWo[g][r] = 0.f;
 #pragma unroll
     for (int k = 0; k < A; ++k) { gbo[k] = 0.f; gls[k] = 0.f; }
     __syncthreads();
@@ -406,13 +435,14 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
       wg_commit();
     }
     // behind the GEMM: warp reduce-scatter of h2[j] * dmu[k] over the 16 rows of this warp (flat (c, k) index, 48 values:
-    // 24 + 12 + 6 shuffles); lane ends with the sums of the flat indices wo_base .. wo_base + 5
-    {
+    // 24 + 12 + 6 shuffles), once per group g of 3 actions; lane ends with the sums of flat indices wo_base .. wo_base + 5
+#pragma unroll
+    for (int g = 0; g < KG; ++g) {
       float dm3[2][3];
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int k = 0; k < 3; ++k) dm3[h][k] = k < A ? dmu[h][k] : 0.f;
+        for (int k = 0; k < 3; ++k) dm3[h][k] = 3 * g + k < A ? dmu[h][3 * g + k] : 0.f;
       auto val = [&](int f) {
         const int c = f / 3, k = f % 3, i = 4 * (c >> 1) + (c & 1);
         return h2f[i] * dm3[0][k] + h2f[i + 2] * dm3[1][k];
@@ -432,8 +462,10 @@ __global__ void __launch_bounds__(U_THREADS, 1) update_umma64_kernel(UpdArgs a) 
 #pragma unroll
       for (int i = 0; i < 6; ++i) {
         const bool up = (lane >> 2) & 1;
-        gWo[i] += (up ? pr[6 + i] : pr[i]) + __shfl_xor_sync(0xffffffffu, up ? pr[i] : pr[6 + i], 4);
+        gWo[g][i] += (up ? pr[6 + i] : pr[i]) + __shfl_xor_sync(0xffffffffu, up ? pr[i] : pr[6 + i], 4);
       }
+    }
+    {
 #pragma unroll
       for (int k = 0; k < A; ++k) {
         const float sdm = warp_sum(t4 == 0 ? dmu[0][k] + dmu[1][k] : 0.f);
