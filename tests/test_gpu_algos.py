@@ -27,6 +27,10 @@ def dev():
 
 
 def _make(env_name):
+    if env_name == "half_cheetah":                 # not one of bench.py's workloads
+        from rllab_b200.envs.mujoco.half_cheetah_env import HalfCheetahEnv
+        from rllab_b200.envs.normalized_env import normalize
+        return normalize(HalfCheetahEnv())
     import bench
     return bench.make_env(env_name)
 
@@ -190,7 +194,11 @@ def test_samples_data_wire_format(dev):
     np.testing.assert_allclose(p0["returns"], S.discount_cumsum(p0["rewards"], 0.99), rtol=1e-5, atol=1e-5)
 
 
-@pytest.mark.parametrize("env_name", ["point", "cartpole", "pendulum", "cartpole_swingup", "double_pendulum", "swimmer", "hopper"])
+PROTOCOL_ENVS = ["point", "cartpole", "pendulum", "cartpole_swingup", "double_pendulum", "swimmer", "hopper",
+                 "half_cheetah"]
+
+
+@pytest.mark.parametrize("env_name", PROTOCOL_ENVS)
 def test_env_protocol(dev, env_name):
     """tests/envs/test_envs.py:86-102: reset in obs space, action in action space, one step, scalar reward."""
     env = _make(env_name)

@@ -24,7 +24,7 @@ pytestmark = pytest.mark.gpu
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 DEV = torch.device("cuda", 0) if torch.cuda.is_available() else None
-ENVS = ["point", "cartpole", "pendulum", "swimmer", "hopper", "cartpole_swingup", "double_pendulum"]
+ENVS = ["point", "cartpole", "pendulum", "swimmer", "hopper", "cartpole_swingup", "double_pendulum", "half_cheetah"]
 
 
 def _L():
@@ -138,7 +138,7 @@ def _pop_and_lanes(kind_name, H, E, M, mpl, seed=11, it=3, lane0=5, check=None):
 @pytest.mark.parametrize("env", ENVS)
 def test_population_rollout_matches_lane_rollout(env, H, E, M):
     # CartPole: random policies fall after 3-20 steps, so a horizon of 12 both cuts and ends episodes
-    mpl = {"cartpole": 12, "swimmer": 60, "hopper": 60}.get(env, 80)
+    mpl = {"cartpole": 12, "swimmer": 60, "hopper": 60, "half_cheetah": 60}.get(env, 80)
     check = None if M <= 77 else sorted(set(list(range(8)) + list(range(M - 8, M)) +
                                             list(np.random.RandomState(M).choice(M, 24, replace=False))))
     ln = _pop_and_lanes(env, H, E, M, mpl, check=check)

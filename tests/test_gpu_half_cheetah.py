@@ -1,5 +1,6 @@
 """HalfCheetah on the GPU against the float64 oracle (tests/planar_tree_oracle.py): env reset / step on lanes in free
-flight, at joint limits, on their feet and upside down on the torso and head; the fused lane rollout at hidden 32 and
+flight, at joint limits, on their feet, upside down on the torso and head, and sunk into the floor with all 38 constraint
+rows active (the compaction arrays full); the fused lane rollout at hidden 32 and
 64, step by step, with the in-kernel Philox stream (action noise chunks 0 and 1) equal to injected noise."""
 import numpy as np
 import pytest
@@ -28,7 +29,9 @@ def dev():
 
 
 def _mixed_states(rng, n):
-    """Four groups of n lanes: airborne, hinges pushed past their limits, standing / landing, flipped onto the back."""
+    """Five groups of n lanes: airborne, hinges pushed past their limits, standing / landing, flipped onto the back, and
+    sunk into the floor with every hinge past a limit (all 38 constraint rows active).  The fifth group draws from its
+    own stream, so the first four and whatever the caller draws from `rng` next do not depend on it."""
     m = T.half_cheetah_model()
     q = np.zeros((9, 4 * n))
     v = rng.normal(0, 1.0, (9, 4 * n))
@@ -48,7 +51,14 @@ def _mixed_states(rng, n):
     q[2, g[3]] = np.pi + rng.uniform(-0.4, 0.4, n)
     q[3:, g[3]] = rng.uniform(lo, hi, (6, n))
     v[:, g[3]] *= 0.3
-    return np.concatenate([q, v]).astype(np.float32)
+    g5 = np.random.RandomState(n + 5)
+    q5 = np.zeros((9, n))
+    q5[0] = g5.uniform(-2, 2, n)
+    q5[1] = g5.uniform(-2.5, -1.0, n)                             # every end sphere below the floor
+    q5[2] = g5.uniform(-0.3, 0.3, n)
+    q5[3:] = np.where(g5.rand(6, n) < 0.5, lo - g5.uniform(0.01, 0.1, (6, n)), hi + g5.uniform(0.01, 0.1, (6, n)))
+    v5 = g5.normal(0, 1.0, (9, n))
+    return np.concatenate([np.concatenate([q, q5], axis=1), np.concatenate([v, v5], axis=1)]).astype(np.float32)
 
 
 def _report(key, err):
@@ -62,7 +72,7 @@ def test_env_step_matches_oracle_on_every_contact_regime(dev):
     n = 512
     s0 = _mixed_states(rng, n)
     N = s0.shape[1]
-    u = rng.uniform(-1.5, 1.5, (6, N)).astype(np.float32)
+    u = np.concatenate([rng.uniform(-1.5, 1.5, (6, 4 * n)), rng.uniform(-1.5, 1.5, (6, n))], axis=1).astype(np.float32)
     env = T.HalfCheetahEnv()
     # the oracle takes the device's action map (NormalizedEnv with lb, ub = -1, 1 clips) on the same float32 inputs
     s_ref, r_ref, d_ref = env.step(s0.astype(np.float64), np.clip(u.astype(np.float64), -1, 1))
@@ -70,6 +80,7 @@ def test_env_step_matches_oracle_on_every_contact_regime(dev):
     assert (kin0["n_active"][2 * n:3 * n] > 0).mean() > 0.85         # most crouched lanes touch the floor
     assert (kin0["n_active"][3 * n:] > 0).all()                      # every flipped lane lies on the floor
     assert (kin0["n_active"][n:2 * n] > 0).all()                     # the limit group has active limit rows
+    assert (kin0["n_active"][4 * n:] == 38).mean() >= 0.99           # the sunk group fills the compaction arrays
     state = torch.tensor(s0, device=dev).contiguous()
     obs = torch.empty((20, N), dtype=torch.float32, device=dev)
     rew = torch.empty(N, dtype=torch.float32, device=dev)
@@ -83,8 +94,8 @@ def test_env_step_matches_oracle_on_every_contact_regime(dev):
     # a residual within float32 rounding of zero can take a different active set, and only those are excused
     near = (np.abs(T.constraint_residuals(env.m, list(s0[:9].astype(np.float64)))) < 1e-5).any(axis=0)
     assert near.mean() < 0.01, near.mean()
-    for k, (lo_, hi_) in enumerate([(0, n), (n, 2 * n), (2 * n, 3 * n), (3 * n, 4 * n)]):
-        name = ["free", "limits", "feet", "flipped"][k]
+    for k, name in enumerate(["free", "limits", "feet", "flipped", "all_rows"]):
+        lo_, hi_ = k * n, (k + 1) * n
         sl = slice(lo_, hi_)
         scale = 1.0 + np.abs(s_ref[:, sl])
         err = np.abs(s1[:, sl] - s_ref[:, sl]) / scale

@@ -43,7 +43,6 @@ import pytest
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
-from oracle import envs as E            # noqa: E402
 from oracle import policy as P          # noqa: E402
 from oracle import sampler as S         # noqa: E402
 from test_gpu_update_shapes import dev, n_sm  # noqa: E402,F401
@@ -439,7 +438,8 @@ def test_solve_retry_and_failure_at_dmax(dev):
 # policy (torques up to +-50) its angular velocities overflow float32 after ~70 steps, and the fit needs finite inputs.
 FIT_ENVS = [("point", 32, 4096, 100), ("cartpole", 32, 2048, 200), ("pendulum", 32, 2048, 200),
             ("cartpole_swingup", 32, 4096, 100), ("double_pendulum", 32, 4096, 40), ("swimmer", 32, 512, 500),
-            ("hopper", 32, 512, 500), ("hopper", 64, 512, 500)]
+            ("hopper", 32, 512, 500), ("hopper", 64, 512, 500), ("half_cheetah", 32, 512, 500),
+            ("half_cheetah", 64, 512, 500)]
 
 
 @pytest.mark.parametrize("env_name,hidden,lanes,T", FIT_ENVS, ids=["%s-%d" % (e[0], e[1]) for e in FIT_ENVS])
@@ -453,25 +453,28 @@ def test_lfb_fit_on_rollout(dev, env_name, hidden, lanes, T):
     Measured on an H100 80GB HBM3 (400 W limit), solve alone / end to end, condition number of A + reg I:
       point 4.3e-14 / 1.0e-7 (4e6), cartpole 3.9e-14 / 4.4e-7 (2e7), pendulum 1.2e-14 / 6.7e-7 (2e10),
       cartpole_swingup 8.5e-14 / 7.5e-7 (1e7), double_pendulum 9.9e-14 / 3.2e-13 (2e14), swimmer 7.0e-12 / 7.4e-12
-      (6e13), hopper-32 5.9e-9 / 6.5e-9 (5e14), hopper-64 3.1e-7 / 4.8e-7 (6e14); one attempt everywhere.  The two
+      (6e13), hopper-32 5.9e-9 / 6.5e-9 (5e14), hopper-64 3.1e-7 / 4.8e-7 (6e14), half_cheetah-32 9.0e-12 / 2.6e-11
+      (4e14), half_cheetah-64 3.2e-11 / 3.2e-11 (3e14; 700 W); one attempt everywhere.  HalfCheetah's obs holds an
+      identically zero column (comY), so two feature columns are zero and A + reg I has the eigenvalue reg exactly.  The two
       solves are backward stable on the same system, so their gap follows the conditioning: 1e-8 holds below κ ~ 1e14,
       Hopper's κ ~ 6e14 takes it to 3.1e-7.  With the float32 tile Gram this module was written against, Hopper's end to
       end figure was 2.8e-4 (hopper-32) and 4.8e-2 (hopper-64), and TRPO's first Hopper-64 fit needed reg 1e-4."""
     ops, L = _ops(), _L()
-    env = E.make(env_name)
-    dims = P.Dims(env.O, (hidden, hidden), env.A)
+    info = L.env_info(L.ENV_KINDS[env_name])
+    O, A = info["obs_dim"], info["act_dim"]
+    dims = P.Dims(O, (hidden, hidden), A)
     theta = P.init_params(dims, np.random.RandomState(5))
-    theta[-env.A:] = -0.5
+    theta[-A:] = -0.5
     th32 = torch.tensor(theta, dtype=torch.float32, device=dev)
-    b = ops.LaneBatch(env.O, env.A, lanes, T, dev)
+    b = ops.LaneBatch(O, A, lanes, T, dev)
     ops.rollout(L.ENV_KINDS[env_name], th32, hidden, hidden, 1e-6, b, T, None, None, 11, 0)
     ops.process_samples(b, None, 0.99, 1.0, drop_cut_paths=True)
-    d1 = 2 * env.O + 5
+    d1 = 2 * O + 5
     gram = torch.empty((d1 * (d1 + 1) // 2,), dtype=torch.float64, device=dev)
     ops.lfb_gram(b, gram)
     w = torch.empty((d1 - 1,), dtype=torch.float64, device=dev)
-    info = torch.zeros((3,), dtype=torch.float64, device=dev)
-    ops.lfb_solve(env.O, gram, REG, w, info)
+    fit = torch.zeros((3,), dtype=torch.float64, device=dev)
+    ops.lfb_solve(O, gram, REG, w, fit)
     traj = b.to_numpy()
     keep = b.valid_mask().reshape(-1)
     F = S.lfb_features_lanes(traj["obs"], traj["tstep"]).reshape(d1 - 1, -1)[:, keep]
@@ -483,14 +486,14 @@ def test_lfb_fit_on_rollout(dev, env_name, hidden, lanes, T):
     e_solve = np.abs(pred - S.lfb_fit_normal(Gd[:-1, :-1], Gd[:-1, -1], REG) @ F).max() / s
     e_fit = np.abs(pred - S.lfb_fit_normal(F @ F.T, F @ y, REG) @ F).max() / s
     print("%s-%d: %d valid samples, cond %.2g, info %s, solve %.3g, end to end %.3g of max|ret| = %.4g" % (
-        env_name, hidden, keep.sum(), np.linalg.cond(Gd[:-1, :-1] + REG * np.eye(d1 - 1)), info.cpu().tolist(),
+        env_name, hidden, keep.sum(), np.linalg.cond(Gd[:-1, :-1] + REG * np.eye(d1 - 1)), fit.cpu().tolist(),
         e_solve, e_fit, s))
-    assert tuple(info.cpu().tolist()) == (REG, 0.0, 1.0)
+    assert tuple(fit.cpu().tolist()) == (REG, 0.0, 1.0)
     assert e_solve <= 1e-6, e_solve
     assert e_fit <= 1e-5, e_fit
 
 
-@pytest.mark.parametrize("env_name,hidden", [("swimmer", 32), ("hopper", 64)])
+@pytest.mark.parametrize("env_name,hidden", [("swimmer", 32), ("hopper", 64), ("half_cheetah", 64)])
 def test_fit_flag_through_trpo(dev, env_name, hidden):
     """Through the plugin API (TRPO + LinearFeatureBaseline, 512 lanes x 500 steps): every iteration's device fit
     succeeds at the first attempt."""
