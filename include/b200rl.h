@@ -48,6 +48,9 @@ extern "C" {
 #define B200RL_ENV_CARTPOLE_SWINGUP 5 /* rllab/envs/box2d/cartpole_swingup_env.py (same Box2D model as CartpoleEnv) */
 #define B200RL_ENV_DOUBLE_PENDULUM 6 /* rllab/envs/box2d/double_pendulum_env.py (models/double_pendulum.xml.mako) */
 #define B200RL_ENV_HALF_CHEETAH 7 /* rllab/envs/mujoco/half_cheetah_env.py (vendor/mujoco_models/half_cheetah.xml) */
+/* GymEnv("CartPole-v0") over gym 0.7.4: Discrete(2) actions.  The action float of env_step is the action index; the
+ * Gaussian b200rl_rollout rejects it, b200rl_rollout_categorical drives it. */
+#define B200RL_ENV_GYM_CARTPOLE 8
 
 #define B200RL_NOISE_UNIFORM 0
 #define B200RL_NOISE_NORMAL 1
@@ -80,6 +83,9 @@ int b200rl_device_sms(int* sms_out);
  * Env.action_space / observation_space of rllab/envs/base.py:43-62. */
 int b200rl_env_info(int env_kind, int* obs_dim, int* act_dim, int* state_dim, int* reset_dim, int* noise_kind,
                     float* lb_host, float* ub_host);
+
+/* *n_out = number of discrete actions of an env kind (its action space is Discrete(n)), 0 for a Box action space. */
+int b200rl_env_num_actions(int env_kind, int* n_out);
 
 /* Number of policy parameters P for (O, h1, h2, A); <0 if the network size is not compiled in. */
 long long b200rl_policy_num_params(int obs_dim, int h1, int h2, int act_dim);
@@ -229,6 +235,68 @@ int b200rl_update_f64(int mode, int loss_kind, const double* params_f64, int obs
                       const float* old_mean, const float* old_log_std, const unsigned char* flags, const double* x,
                       double scale, const double* count, double reg_coeff, double diag_scale, double* vec_out,
                       double* loss_out, double* ws, void* stream);
+
+/* ---- CategoricalMLPPolicy (rllab/policies/categorical_mlp_policy.py, rllab/distributions/categorical.py).  Net: tanh
+ * (h1, h2) trunk, softmax output over n actions; flat layout [W0 (O,h1), b0, W1 (h1,h2), b1, Wout (h2,n), bout], no log_std
+ * (P = O*h1+h1 + h1*h2+h2 + h2*n+n).  Compiled for O = 4, hidden (32,32), n = 2 (CartPole-v0); any other shape returns
+ * B200RL_EUNSUPPORTED.  Lane layout as above with A = n: act [n][T][N] holds the ONE-HOT action (the reference's
+ * flattened action), the mean planes hold prob [n][T][N].  The update passes take `act` one-hot and `old_prob` [n][B], and
+ * follow the conventions of b200rl_loss_kl / b200rl_grad / b200rl_fvp (flags, scale, count, fixed-order reductions,
+ * peer fusion); probabilities are softmax(z) (max-shifted, ascending-k sum) after the rollout's forward in every pass, so
+ * the likelihood ratio is exactly 1 and the KL exactly 0 at theta_old. ---- */
+long long b200rl_categorical_num_params(int obs_dim, int h1, int h2, int n_actions);
+
+/* CategoricalMLPPolicy.get_actions: obs [O][n] -> act_out [n] int32 action indices = weighted_sample(prob, u)
+ * (#{k : cumsum_k(prob) < u}, clipped to n_actions-1; rllab/misc/special.py:10-19), prob_out [n_actions][n].  u [n] or
+ * NULL (Philox stream 0 at (lane0 + i, row), the first word of the uniform map, as b200rl_fill_noise with K = 1). */
+int b200rl_categorical_get_actions(const float* params_f32, int obs_dim, int h1, int h2, int n_actions,
+                                   const float* obs, long long n, const float* u, unsigned int seed, unsigned int iter,
+                                   int row, long long lane0, int* act_out, float* prob_out, void* stream);
+
+/* Fused rollout of a discrete-action env kind with a categorical policy: b200rl_rollout's lane semantics (auto-reset,
+ * FLAG_DONE / FLAG_END / FLAG_CUT, tstep), with the action drawn as in b200rl_categorical_get_actions from u [T][N]
+ * (tests) or NULL = Philox stream 0 row t.  Writes obs, one-hot act [n][T][N], prob [n][T][N], rew, flags, tstep. */
+int b200rl_rollout_categorical(int env_kind, const float* params_f32, int h1, int h2, int N, int T,
+                               int max_path_length, const float* u, const float* reset_raw, unsigned int seed,
+                               unsigned int iter, long long lane0, float* obs, float* act, float* prob, float* rew,
+                               unsigned char* flags, unsigned short* tstep, void* stream);
+
+/* (loss, sum KL, max KL) as b200rl_loss_kl: TRPO  -adv (p_new.x + 1e-8) / (p_old.x + 1e-8),  VPG  -adv log(p.x + 1e-8),
+ * KL = sum_k p_old (log(p_old + 1e-8) - log(p_new + 1e-8)) (categorical.py). */
+int b200rl_categorical_loss_kl(int loss_kind, const float* params_f32, int obs_dim, int h1, int h2, int n_actions,
+                               long long B, const float* obs, const float* act, const float* adv,
+                               const float* old_prob, const unsigned char* flags, double scale, const double* count,
+                               double* out, double* ws, void* stream);
+
+/* Gradient of the surrogate plus penalty * mean KL (penalty 0: b200rl_grad, > 0: b200rl_grad_penalized); loss_out (3 or
+ * NULL) = the unpenalised triple of the same pass, h_cache_out ([h1+h2][B] or NULL) the hidden activations. */
+int b200rl_categorical_grad(int loss_kind, double penalty, const float* params_f32, int obs_dim, int h1, int h2,
+                            int n_actions, long long B, const float* obs, const float* act, const float* adv,
+                            const float* old_prob, const unsigned char* flags, double scale, const double* count,
+                            double* g_out, double* loss_out, float* h_cache_out, double* ws, void* stream);
+
+/* Fisher-vector product J^T M J x (+ diag_scale * reg_coeff * x) at theta_old, M = Hessian of the per-sample KL in the
+ * logits at theta_old with the 1e-8 kept (DESIGN.md section 5); arguments as b200rl_fvp. */
+int b200rl_categorical_fvp(const float* params_f32, int obs_dim, int h1, int h2, int n_actions, long long B,
+                           const float* obs, const unsigned char* flags, const double* x, double scale,
+                           const double* count, double reg_coeff, double diag_scale, double* Hx_out,
+                           const float* h_cache, const int* tile_list, int n_list, double* ws, void* stream);
+
+/* float64 parity mode of the three passes above on the float64 master parameters, as b200rl_update_f64 (mode 0 loss/KL
+ * -> loss_out[3], 1 gradient -> vec_out[P] (+ loss_out), 2 Fisher-vector product of x -> vec_out[P]); loss_kind
+ * B200RL_LOSS_KL with mode 1 is the gradient of mean KL(old || new) (FiniteDifferenceHvp).  Mode 2 is the exact Hessian
+ * of mean KL at theta_old, including the O(1e-8) term of the KL's first derivative in the logits that the float32 pass
+ * leaves out (DESIGN.md section 5).  Weight gradients are summed with float64 atomics: reruns agree to rounding. */
+int b200rl_categorical_update_f64(int mode, int loss_kind, const double* params_f64, int obs_dim, int h1, int h2,
+                                  int n_actions, long long B, const float* obs, const float* act, const float* adv,
+                                  const float* old_prob, const unsigned char* flags, const double* x, double scale,
+                                  const double* count, double reg_coeff, double diag_scale, double* vec_out,
+                                  double* loss_out, double* ws, void* stream);
+
+/* out [2] float64 = (sum over valid samples of -sum_k p_k log(p_k + 1e-8), number of valid samples) of prob [n][B]
+ * (categorical.py:entropy; the sampler's Entropy is out[0] / out[1] after the all-reduce). */
+int b200rl_categorical_entropy(int n_actions, long long B, const float* prob, const unsigned char* flags, double* out,
+                               double* ws, void* stream);
 
 /* ---- GaussianMLPRegressor, the value function of GaussianMLPBaseline (rllab/regressors/gaussian_mlp_regressor.py,
  * rllab/baselines/gaussian_mlp_baseline.py).  Net: MLP(obs_dim -> h1 -> h2 -> 1), ReLU hidden units, no output

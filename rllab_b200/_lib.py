@@ -16,6 +16,10 @@ ENV_HALF_CHEETAH = 7
 ENV_KINDS = dict(point=ENV_POINT, cartpole=ENV_CARTPOLE, pendulum=ENV_PENDULUM, swimmer=ENV_SWIMMER, hopper=ENV_HOPPER,
                  cartpole_swingup=ENV_CARTPOLE_SWINGUP, double_pendulum=ENV_DOUBLE_PENDULUM,
                  half_cheetah=ENV_HALF_CHEETAH)
+# Discrete-action env kinds (b200rl_env_num_actions > 0): driven by the categorical rollout only, so they are kept out of
+# ENV_KINDS, the Box-action kinds every Gaussian test grid covers.
+ENV_GYM_CARTPOLE = 8
+DISCRETE_ENV_KINDS = dict(gym_cartpole=ENV_GYM_CARTPOLE)
 NOISE_UNIFORM, NOISE_NORMAL = 0, 1
 LOSS_TRPO, LOSS_VPG, LOSS_KL = 0, 1, 2
 FLAG_DONE, FLAG_END, FLAG_CUT, FLAG_MASKED = 1, 2, 4, 8
@@ -33,6 +37,7 @@ SIGNATURES = {
     "b200rl_bench_ffma2": (c_int, [c_int, _P, POINTER(_LL), _P]),
     "b200rl_env_info": (c_int, [c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int), POINTER(c_int),
                                 POINTER(c_float), POINTER(c_float)]),
+    "b200rl_env_num_actions": (c_int, [c_int, POINTER(c_int)]),
     "b200rl_policy_num_params": (_LL, [c_int, c_int, c_int, c_int]),
     "b200rl_fill_noise": (c_int, [_P, c_int, c_int, c_int, c_int, _LL, c_int, c_uint, c_uint, c_int, _P]),
     "b200rl_env_reset": (c_int, [c_int, c_int, _P, _P, _P, c_uint, c_uint, c_int, _LL, _P]),
@@ -89,6 +94,20 @@ SIGNATURES = {
     "b200rl_rows_mean_std": (c_int, [_LL, c_int, _P, _P, _P, _P]),
     "b200rl_reps_delta_max": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, c_int, _P, _P, _P, _P]),
     "b200rl_reps_dual_sums": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, c_int, _P, c_double, _P, _P, _P, _P, _P]),
+    "b200rl_categorical_num_params": (_LL, [c_int, c_int, c_int, c_int]),
+    "b200rl_categorical_get_actions": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _LL, _P, c_uint, c_uint, c_int, _LL,
+                                               _P, _P, _P]),
+    "b200rl_rollout_categorical": (c_int, [c_int, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_uint, c_uint, _LL,
+                                           _P, _P, _P, _P, _P, _P, _P]),
+    "b200rl_categorical_loss_kl": (c_int, [c_int, _P, c_int, c_int, c_int, c_int, _LL, _P, _P, _P, _P, _P, c_double, _P,
+                                           _P, _P, _P]),
+    "b200rl_categorical_grad": (c_int, [c_int, c_double, _P, c_int, c_int, c_int, c_int, _LL, _P, _P, _P, _P, _P,
+                                        c_double, _P, _P, _P, _P, _P, _P]),
+    "b200rl_categorical_fvp": (c_int, [_P, c_int, c_int, c_int, c_int, _LL, _P, _P, _P, c_double, _P, c_double, c_double,
+                                       _P, _P, _P, c_int, _P, _P]),
+    "b200rl_categorical_entropy": (c_int, [c_int, _LL, _P, _P, _P, _P, _P]),
+    "b200rl_categorical_update_f64": (c_int, [c_int, c_int, _P, c_int, c_int, c_int, c_int, _LL, _P, _P, _P, _P, _P,
+                                              _P, c_double, _P, c_double, c_double, _P, _P, _P, _P]),
 }
 
 _lib = None
@@ -165,3 +184,18 @@ def vf_num_params(O, h1=32, h2=32):
     if n < 0:
         raise B200RLError("unsupported regressor network O=%d hidden=(%d,%d): %s" % (O, h1, h2, last_error()))
     return int(n)
+
+
+def env_num_actions(kind):
+    """Number of discrete actions of an env kind (its action space is Discrete(n)); 0 for a Box action space."""
+    lib = load()
+    n = c_int()
+    check(lib.b200rl_env_num_actions(kind, n), "b200rl_env_num_actions")
+    return n.value
+
+
+def categorical_num_params(O, h1, h2, n):
+    p = load().b200rl_categorical_num_params(O, h1, h2, n)
+    if p < 0:
+        raise B200RLError("unsupported categorical network O=%d hidden=(%d,%d) n=%d: %s" % (O, h1, h2, n, last_error()))
+    return int(p)

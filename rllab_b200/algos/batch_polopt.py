@@ -74,8 +74,10 @@ class BatchPolopt(RLAlgorithm):
         b = getattr(paths, "lane_batch", None)
         if b is not None:
             from .. import ops
-            p_ls = ops.PendingHost(b.log_std)          # read back when the table is dumped
-            logger.record_tabular('AveragePolicyStd', lambda: float(np.mean(np.exp(p_ls.get().astype(np.float64)))))
+            if not b.categorical:                     # CategoricalMLPPolicy logs no diagnostics (policies/base.py)
+                p_ls = ops.PendingHost(b.log_std)          # read back when the table is dumped
+                logger.record_tabular('AveragePolicyStd',
+                                      lambda: float(np.mean(np.exp(p_ls.get().astype(np.float64)))))
             if self.store_paths:
                 self.env.log_diagnostics(paths.to_paths())
         else:

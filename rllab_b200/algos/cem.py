@@ -67,6 +67,9 @@ class CEM(RLAlgorithm, Serializable):
         Serializable.quick_init(self, locals())
         if plot:
             raise NotImplementedError("plotting is outside the B200 hot path")
+        from .. import ops
+        if ops.is_categorical(getattr(policy, "dims", None)):
+            raise NotImplementedError("CEM's population rollout is built for GaussianMLPPolicy only")
         self.env = env
         self.policy = policy
         self.batch_size = batch_size

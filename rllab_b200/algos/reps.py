@@ -23,7 +23,8 @@ every function evaluation is one pass over the lane batch on the GPU:
 Regularizable parameters (the L2_reg_loss term, reps.py:115-118): lasagne's Layer.add_param tags every parameter
 regularizable unless told otherwise; DenseLayer adds its bias with regularizable=False; rllab's ParamLayer
 (core/lasagne_layers.py:15) adds the log_std parameter with the defaults.  So for GaussianMLPPolicy they are W0, W1,
-Wout and log_std (n_reg = 4), and the term is L2_reg_loss * sum_p mean(p^2) / 4.
+Wout and log_std (n_reg = 4), and the term is L2_reg_loss * sum_p mean(p^2) / 4; CategoricalMLPPolicy has no log_std, so
+its regularizable parameters are W0, W1 and Wout (n_reg = 3).
 
 Multi-GPU: the maximum and the sums are all-reduced through the Comm (max, then sums), and the policy passes through
 PolicyObjective's reduction, so every rank hands scipy identical numbers and theta, eta and v are bit-identical across
@@ -67,12 +68,14 @@ def dual_from_sums(eta, M, sums, count, epsilon, l2_reg_dual):
 
 
 def regularizable_slices(policy):
-    """Flat-parameter slices of W0, W1, Wout and log_std (see the module docstring)."""
+    """Flat-parameter slices of the weight matrices and, for GaussianMLPPolicy, log_std (see the module docstring)."""
+    from .. import ops
+    has_log_std = not ops.is_categorical(getattr(policy, "dims", None))
     out, k = [], 0
     shapes = policy.get_param_shapes()
     for i, s in enumerate(shapes):
         n = int(np.prod(s))
-        if len(s) == 2 or i == len(shapes) - 1:
+        if len(s) == 2 or (has_log_std and i == len(shapes) - 1):
             out.append(slice(k, k + n))
         k += n
     return out

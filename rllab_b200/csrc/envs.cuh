@@ -189,6 +189,53 @@ struct PendulumEnvD {
   }
 };
 
+// ---------------------------------------------------------------- gym 0.7.4 CartPole-v0 via rllab/envs/gym_env.py
+// gym/envs/classic_control/cartpole.py restated (no in-tree reference dynamics, as Pendulum-v0): explicit Euler with
+// tau = 0.02, the cart moved with the OLD velocities; action index 1 pushes with +10, 0 with -10.  done when |x| > 2.4 or
+// |theta| > 12 deg; reward 1 on every step, the terminal one included.  The single action float is the index
+// (NACT = 2 actions): NormalizedEnv passes a Discrete action through unscaled (normalized_env.py:71-75).
+struct GymCartPoleEnvD {
+  static constexpr int KIND = B200RL_ENV_GYM_CARTPOLE, O = 4, A = 1, S = 4, K = 4, NOISE = B200RL_NOISE_UNIFORM,
+                       NACT = 2;
+  __host__ __device__ static constexpr float lb(int) { return 0.0f; }
+  __host__ __device__ static constexpr float ub(int) { return (float)(NACT - 1); }
+  __device__ static void reset(float (&s)[S], const float (&raw)[K]) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) s[i] = -0.05f + 0.1f * raw[i];    // np_random.uniform(-0.05, 0.05, size=(4,))
+  }
+  __device__ static void obs(const float (&s)[S], float (&o)[O]) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) o[i] = s[i];
+  }
+  __device__ static void step(float (&s)[S], const float (&u)[A], float& r, bool& done) {
+    const float g = 9.8f, mp = 0.1f, total = 1.1f, l = 0.5f, pml = 0.05f, tau = 0.02f;
+    const float thr = 12.0f * 2.0f * 3.14159265358979323846f / 360.0f;
+    const float x = s[0], xd = s[1], th = s[2], thd = s[3];
+    const float force = ((int)u[0] == 1) ? 10.0f : -10.0f;
+    float sn, cs;
+    sincosf(th, &sn, &cs);
+    const float temp = (force + pml * thd * thd * sn) / total;
+    const float thacc = (g * sn - cs * temp) / (l * (4.0f / 3.0f - mp * cs * cs / total));
+    const float xacc = temp - pml * thacc * cs / total;
+    s[0] = x + tau * xd;
+    s[1] = xd + tau * xacc;
+    s[2] = th + tau * thd;
+    s[3] = thd + tau * thacc;
+    done = (s[0] < -2.4f) || (s[0] > 2.4f) || (s[2] < -thr) || (s[2] > thr);
+    r = 1.0f;
+  }
+};
+
+// Number of discrete actions of an env kind: Env::NACT where the struct declares it, 0 for a Box action space.
+template <class Env, class = void>
+struct EnvNumActions {
+  static constexpr int value = 0;
+};
+template <class Env>
+struct EnvNumActions<Env, std::void_t<decltype(Env::NACT)>> {
+  static constexpr int value = Env::NACT;
+};
+
 }  // namespace b200rl
 
 #include "planar.cuh"
@@ -273,5 +320,14 @@ __device__ __forceinline__ void draw_eps(float (&e)[A], const float* __restrict_
       ::b200rl::set_error("unknown env kind %d", (int)(kind));                                \
       return B200RL_EUNSUPPORTED;                                                             \
   }
+
+// B200RL_DISPATCH_ENV plus the discrete-action kinds (Env::A = 1 float holding the action index).  For the entry points
+// that take any env (info, reset, step); the Gaussian rollout and the population rollout dispatch Box kinds only.
+#define B200RL_DISPATCH_ENV_ANY(kind, ...)                                                    \
+  if ((kind) == B200RL_ENV_GYM_CARTPOLE) {                                                    \
+    using Env = ::b200rl::GymCartPoleEnvD;                                                    \
+    __VA_ARGS__;                                                                              \
+  } else                                                                                      \
+    B200RL_DISPATCH_ENV(kind, __VA_ARGS__)
 
 }  // namespace b200rl

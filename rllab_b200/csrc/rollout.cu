@@ -121,7 +121,8 @@ __global__ void env_step_kernel(int N, int normalized, float* __restrict__ state
 #pragma unroll
   for (int k = 0; k < Env::A; ++k) {
     const float a = actions[(size_t)k * N + n];
-    u[k] = normalized ? scale_action(a, Env::lb(k), Env::ub(k)) : a;
+    // a discrete action (an index) passes NormalizedEnv unscaled (normalized_env.py:71-75)
+    u[k] = (normalized && EnvNumActions<Env>::value == 0) ? scale_action(a, Env::lb(k), Env::ub(k)) : a;
   }
   float r;
   bool done;
@@ -213,7 +214,7 @@ extern "C" {
 
 int b200rl_env_info(int env_kind, int* obs_dim, int* act_dim, int* state_dim, int* reset_dim, int* noise_kind,
                     float* lb_host, float* ub_host) {
-  B200RL_DISPATCH_ENV(env_kind, {
+  B200RL_DISPATCH_ENV_ANY(env_kind, {
     if (obs_dim) *obs_dim = Env::O;
     if (act_dim) *act_dim = Env::A;
     if (state_dim) *state_dim = Env::S;
@@ -224,6 +225,12 @@ int b200rl_env_info(int env_kind, int* obs_dim, int* act_dim, int* state_dim, in
       if (ub_host) ub_host[k] = Env::ub(k);
     }
   });
+  return 0;
+}
+
+int b200rl_env_num_actions(int env_kind, int* n_out) {
+  B200RL_REQUIRE(n_out, "env_num_actions: null output");
+  B200RL_DISPATCH_ENV_ANY(env_kind, { *n_out = EnvNumActions<Env>::value; });
   return 0;
 }
 
@@ -251,7 +258,7 @@ int b200rl_fill_noise(float* out, int rows, int row0, int K, int N, long long la
 int b200rl_env_reset(int env_kind, int N, float* state, float* obs_out, const float* reset_raw, unsigned int seed,
                      unsigned int iter, int row, long long lane0, void* stream) {
   B200RL_REQUIRE(N > 0 && state && obs_out, "env_reset: bad arguments");
-  B200RL_DISPATCH_ENV(env_kind, {
+  B200RL_DISPATCH_ENV_ANY(env_kind, {
     env_reset_kernel<Env><<<(N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(N, state, obs_out, reset_raw, seed,
                                                                               iter, row, lane0);
   });
@@ -262,7 +269,7 @@ int b200rl_env_reset(int env_kind, int N, float* state, float* obs_out, const fl
 int b200rl_env_step(int env_kind, int N, int normalized, float* state, const float* actions, float* obs_out,
                     float* rew_out, unsigned char* done_out, void* stream) {
   B200RL_REQUIRE(N > 0 && state && actions && obs_out && rew_out && done_out, "env_step: bad arguments");
-  B200RL_DISPATCH_ENV(env_kind, {
+  B200RL_DISPATCH_ENV_ANY(env_kind, {
     env_step_kernel<Env><<<(N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(N, normalized, state, actions, obs_out,
                                                                              rew_out, done_out);
   });
@@ -293,6 +300,8 @@ int b200rl_rollout(int env_kind, const float* params_f32, int h1, int h2, float 
   B200RL_REQUIRE(N > 0 && T > 0 && max_path_length > 0, "rollout: N, T, max_path_length must be positive");
   B200RL_REQUIRE(max_path_length <= 65535, "rollout: max_path_length must fit uint16 tstep");
   B200RL_REQUIRE(h1 == h2, "rollout: hidden sizes must be equal (32,32) or (64,64)");
+  B200RL_REQUIRE(env_kind != B200RL_ENV_GYM_CARTPOLE,
+                 "rollout: env kind %d has a discrete action space (b200rl_rollout_categorical drives it)", env_kind);
   RolloutArgs a;
   a.params = params_f32;
   a.log_min_std = min_std > 0.f ? logf(min_std) : -INFINITY;

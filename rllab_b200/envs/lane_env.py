@@ -11,7 +11,7 @@ There is no CPU fallback: constructing an env needs libb200rl.so, stepping it ne
 import numpy as np
 
 from .. import _lib as L
-from ..spaces import Box
+from ..spaces import Box, Discrete
 from .base import Env, Step
 
 BIG = 1e6
@@ -41,8 +41,9 @@ class LaneEnv(Env):
     HORIZON = None
 
     def __init__(self):
-        self.env_kind = L.ENV_KINDS[self.ENV_NAME]
+        self.env_kind = L.ENV_KINDS[self.ENV_NAME] if self.ENV_NAME in L.ENV_KINDS else L.DISCRETE_ENV_KINDS[self.ENV_NAME]
         self._info = L.env_info(self.env_kind)
+        self._n_actions = L.env_num_actions(self.env_kind)
         self._one = None          # lazily created one-lane device buffers
         self._normalized = False  # toggled by NormalizedEnv
 
@@ -54,6 +55,8 @@ class LaneEnv(Env):
 
     @property
     def action_space(self):
+        if self._n_actions > 0:             # the action is an index: env_step reads it as one float
+            return Discrete(self._n_actions)
         return Box(np.array(self._info["lb"], dtype=np.float64), np.array(self._info["ub"], dtype=np.float64))
 
     @property

@@ -72,6 +72,7 @@ class LaneBatch(object):
         self.processed = False        # adv/ret/base valid (process_samples has run on this rollout)
         self.B_global = N * T         # samples over all ranks (the sampler overwrites it under torchrun)
         self.masked = False           # process_samples dropped cut paths: passes read FLAG_MASKED and the device count
+        self.categorical = False      # act holds one-hot actions and mean the probabilities of a categorical policy
 
     @property
     def B(self):
@@ -99,6 +100,33 @@ class LaneBatch(object):
                     log_std=self.log_std.cpu().numpy())
 
 
+class CategoricalDims(tuple):
+    """(O, h1, h2, n) of a CategoricalMLPPolicy.  A policy hands its `dims` to the update passes below; this type is what
+    makes them run the categorical kernels (b200rl_categorical_*), with batch.mean holding the old probabilities and
+    batch.act the one-hot actions.  A plain tuple (O, h1, h2, A) selects the Gaussian kernels."""
+
+    def __new__(cls, O, h1, h2, n):
+        return tuple.__new__(cls, (int(O), int(h1), int(h2), int(n)))
+
+    def __getnewargs__(self):
+        return tuple(self)
+
+
+def is_categorical(dims):
+    return isinstance(dims, CategoricalDims)
+
+
+_n_actions = {}
+
+
+def env_num_actions(kind):
+    """Discrete actions of an env kind (0: Box), cached per kind."""
+    n = _n_actions.get(kind)
+    if n is None:
+        n = _n_actions[kind] = L.env_num_actions(kind)
+    return n
+
+
 def fill_noise(out, rows, row0, K, N, lane0, kind, seed, it, stream_id):
     _chk(out, F32, "out", rows * K * N)
     L.call("b200rl_fill_noise", L.ptr(out), rows, row0, K, N, lane0, kind, seed, it, stream_id, _stream())
@@ -124,11 +152,36 @@ def policy_get_actions(params32, O, h1, h2, A, min_std, obs, n, eps, seed, it, r
 
 
 def rollout(kind, params32, h1, h2, min_std, batch, max_path_length, eps=None, reset_raw=None, seed=0, it=0, lane0=0):
+    """Fused rollout.  A discrete-action env kind runs the categorical rollout: `eps` is then the injected uniform u
+    [T][N] of the action draw, batch.act receives one-hot actions and batch.mean the probabilities."""
     b = batch
     _chk(params32, F32, "params32"), _chk(eps, F32, "eps"), _chk(reset_raw, F32, "reset_raw")
+    if env_num_actions(kind) > 0:
+        _chk(eps, F32, "u", b.T * b.N)
+        L.call("b200rl_rollout_categorical", kind, L.ptr(params32), h1, h2, b.N, b.T, max_path_length, L.ptr(eps),
+               L.ptr(reset_raw), seed, it, lane0, L.ptr(b.obs), L.ptr(b.act), L.ptr(b.mean), L.ptr(b.rew),
+               L.ptr(b.flags), L.ptr(b.tstep), _stream())
+        return
     L.call("b200rl_rollout", kind, L.ptr(params32), h1, h2, float(min_std or 0.0), b.N, b.T, max_path_length,
            L.ptr(eps), L.ptr(reset_raw), seed, it, lane0, L.ptr(b.obs), L.ptr(b.act), L.ptr(b.mean), L.ptr(b.rew),
            L.ptr(b.flags), L.ptr(b.tstep), L.ptr(b.log_std), _stream())
+
+
+def categorical_get_actions(params32, dims, obs, n, u, seed, it, row, lane0, act_out, prob_out):
+    """act_out [n] int32 = weighted_sample(prob, u), prob_out [n_actions][n] (b200rl_categorical_get_actions)."""
+    O, h1, h2, A = dims
+    _chk(params32, F32, "params32"), _chk(obs, F32, "obs", O * n), _chk(u, F32, "u", n)
+    _chk(act_out, torch.int32, "act_out", n), _chk(prob_out, F32, "prob_out", A * n)
+    L.call("b200rl_categorical_get_actions", L.ptr(params32), O, h1, h2, A, L.ptr(obs), n, L.ptr(u), seed, it, row,
+           lane0, L.ptr(act_out), L.ptr(prob_out), _stream())
+
+
+def categorical_entropy(batch, out):
+    """out [2] float64 = (sum of the entropy of batch.mean's probabilities, number of samples) over the valid samples."""
+    b = batch
+    _chk(out, F64, "out", 2)
+    L.call("b200rl_categorical_entropy", b.A, b.B, L.ptr(b.mean), L.ptr(b.flags) if b.masked else None, L.ptr(out),
+           L.ptr(workspace(b.device)), _stream())
 
 
 def process_samples(batch, w, discount, gae_lambda, drop_cut_paths=False):
@@ -238,6 +291,12 @@ def loss_kl(loss_kind, params32, dims, min_std, batch, out, fuse=False):
     b = batch
     fl, scale, cnt = _mask(b)
     _chk(params32, F32, "params32"), _chk(out, F64, "out", 3)
+    if is_categorical(dims):
+        with _Fused(fuse):
+            L.call("b200rl_categorical_loss_kl", loss_kind, L.ptr(params32), O, h1, h2, A, b.B, L.ptr(b.obs),
+                   L.ptr(b.act), L.ptr(b.adv), L.ptr(b.mean), fl, scale, cnt, L.ptr(out), L.ptr(workspace(b.device)),
+                   _stream())
+        return
     with _Fused(fuse):
         L.call("b200rl_loss_kl", loss_kind, L.ptr(params32), O, h1, h2, A, float(min_std or 0.0), b.B, L.ptr(b.obs),
                L.ptr(b.act), L.ptr(b.adv), L.ptr(b.mean), L.ptr(b.log_std), fl, scale, cnt, L.ptr(out),
@@ -249,6 +308,9 @@ def grad(loss_kind, params32, dims, min_std, batch, g_out, loss_out=None, h_cach
     b = batch
     fl, scale, cnt = _mask(b)
     _chk(params32, F32, "params32"), _chk(g_out, F64, "g_out")
+    if is_categorical(dims):
+        _categorical_grad(loss_kind, 0.0, params32, dims, b, g_out, loss_out, h_cache, fuse)
+        return
     with _Fused(fuse):
         L.call("b200rl_grad", loss_kind, L.ptr(params32), O, h1, h2, A, float(min_std or 0.0), b.B, L.ptr(b.obs),
                L.ptr(b.act), L.ptr(b.adv), L.ptr(b.mean), L.ptr(b.log_std), fl, scale, cnt, L.ptr(g_out), L.ptr(loss_out),
@@ -262,10 +324,23 @@ def grad_penalized(loss_kind, penalty, params32, dims, min_std, batch, g_out, lo
     b = batch
     fl, scale, cnt = _mask(b)
     _chk(params32, F32, "params32"), _chk(g_out, F64, "g_out")
+    if is_categorical(dims):
+        _categorical_grad(loss_kind, penalty, params32, dims, b, g_out, loss_out, None, fuse)
+        return
     with _Fused(fuse):
         L.call("b200rl_grad_penalized", loss_kind, float(penalty), L.ptr(params32), O, h1, h2, A, float(min_std or 0.0),
                b.B, L.ptr(b.obs), L.ptr(b.act), L.ptr(b.adv), L.ptr(b.mean), L.ptr(b.log_std), fl, scale, cnt,
                L.ptr(g_out), L.ptr(loss_out), L.ptr(workspace(b.device)), _stream())
+
+
+def _categorical_grad(loss_kind, penalty, params32, dims, batch, g_out, loss_out, h_cache, fuse):
+    O, h1, h2, A = dims
+    b = batch
+    fl, scale, cnt = _mask(b)
+    with _Fused(fuse):
+        L.call("b200rl_categorical_grad", loss_kind, float(penalty), L.ptr(params32), O, h1, h2, A, b.B, L.ptr(b.obs),
+               L.ptr(b.act), L.ptr(b.adv), L.ptr(b.mean), fl, scale, cnt, L.ptr(g_out), L.ptr(loss_out),
+               L.ptr(h_cache), L.ptr(workspace(b.device)), _stream())
 
 
 def fvp(params32, dims, min_std, batch, x, reg_coeff, diag_scale, Hx_out, h_cache=None, tile_list=None, count=None,
@@ -278,6 +353,12 @@ def fvp(params32, dims, min_std, batch, x, reg_coeff, diag_scale, Hx_out, h_cach
     if tile_list is not None:
         scale, cnt = 1.0, L.ptr(count)
     _chk(params32, F32, "params32"), _chk(x, F64, "x"), _chk(Hx_out, F64, "Hx_out", x.numel())
+    if is_categorical(dims):
+        with _Fused(fuse):
+            L.call("b200rl_categorical_fvp", L.ptr(params32), O, h1, h2, A, b.B, L.ptr(b.obs), fl, L.ptr(x), scale, cnt,
+                   float(reg_coeff), float(diag_scale), L.ptr(Hx_out), L.ptr(h_cache), L.ptr(tile_list),
+                   0 if tile_list is None else int(tile_list.numel()), L.ptr(workspace(b.device)), _stream())
+        return
     with _Fused(fuse):
         L.call("b200rl_fvp", L.ptr(params32), O, h1, h2, A, float(min_std or 0.0), b.B, L.ptr(b.obs), fl, L.ptr(x), scale,
                cnt, float(reg_coeff), float(diag_scale), L.ptr(Hx_out), L.ptr(h_cache), L.ptr(tile_list),
@@ -296,6 +377,12 @@ def update_f64(mode, loss_kind, params64, dims, min_std, batch, x, reg_coeff, di
     b = batch
     fl, scale, cnt = _mask(b)
     _chk(params64, F64, "params64"), _chk(x, F64, "x"), _chk(vec_out, F64, "vec_out"), _chk(loss_out, F64, "loss_out", 3)
+    if is_categorical(dims):
+        with _Fused(fuse):
+            L.call("b200rl_categorical_update_f64", mode, loss_kind, L.ptr(params64), O, h1, h2, A, b.B, L.ptr(b.obs),
+                   L.ptr(b.act), L.ptr(b.adv), L.ptr(b.mean), fl, L.ptr(x), scale, cnt, float(reg_coeff),
+                   float(diag_scale), L.ptr(vec_out), L.ptr(loss_out), L.ptr(workspace(b.device)), _stream())
+        return
     with _Fused(fuse):
         L.call("b200rl_update_f64", mode, loss_kind, L.ptr(params64), O, h1, h2, A, float(min_std or 0.0), b.B, L.ptr(b.obs),
                L.ptr(b.act), L.ptr(b.adv), L.ptr(b.mean), L.ptr(b.log_std), fl, L.ptr(x), scale, cnt, float(reg_coeff),

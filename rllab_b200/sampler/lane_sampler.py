@@ -54,7 +54,8 @@ class LanePaths(object):
 def lanes_to_paths(batch, whole_paths=True):
     """Device lanes -> list of path dicts {observations (L,O), actions (L,A), rewards (L,), agent_infos{mean,log_std},
     env_infos{}} (+ advantages / returns when process_samples has run), lane-major then time order.  whole_paths: leave
-    out the paths cut by the end of the lane buffer (FLAG_CUT on their last sample)."""
+    out the paths cut by the end of the lane buffer (FLAG_CUT on their last sample).  A categorical batch has one-hot
+    actions (L,n) and agent_infos{prob}."""
     t = batch.to_numpy()
     O, T, N = t["obs"].shape
     A = t["act"].shape[0]
@@ -74,7 +75,8 @@ def lanes_to_paths(batch, whole_paths=True):
                 observations=t["obs"][:, sl, n].T.astype(np.float64),
                 actions=t["act"][:, sl, n].T.astype(np.float64),
                 rewards=t["rew"][sl, n].astype(np.float64),
-                agent_infos=dict(mean=t["mean"][:, sl, n].T.astype(np.float64), log_std=np.tile(ls, (e + 1 - start, 1))),
+                agent_infos=(dict(prob=t["mean"][:, sl, n].T.astype(np.float64)) if batch.categorical else
+                             dict(mean=t["mean"][:, sl, n].T.astype(np.float64), log_std=np.tile(ls, (e + 1 - start, 1)))),
                 env_infos=dict(),
             )
             if adv is not None:
@@ -114,6 +116,8 @@ class SamplesData(dict):
             v = rows(b.act, b.A)
         elif key in ("rewards", "returns", "advantages"):
             v = rows(dict(rewards=b.rew, returns=b.ret, advantages=b.adv)[key], 1).reshape(-1)
+        elif key == "agent_infos" and b.categorical:
+            v = dict(prob=rows(b.mean, b.A))
         elif key == "agent_infos":
             v_mean = rows(b.mean, b.A)
             v = dict(mean=v_mean,
@@ -166,6 +170,9 @@ class LaneSampler(Sampler):
             raise ValueError("fewer lanes (%d) than ranks (%d)" % (n_total, self.comm.world_size))
         pol = algo.policy
         self.batch = ops.LaneBatch(pol.obs_dim, pol.action_dim, n_local, T, dev)
+        self.batch.categorical = ops.is_categorical(pol.dims)
+        if self.batch.categorical != (ops.env_num_actions(self.env_kind) > 0):
+            raise TypeError("the policy's action distribution does not match the env's action space")
         self.batch.B_global = n_total * T
         self.batch.processed = False
         self.lane0 = lane0
@@ -228,12 +235,27 @@ class LaneSampler(Sampler):
 
         # statistics: queued pinned-memory readbacks, resolved when the logger dumps the table (or `stats` is read), so
         # the host does not stall the GPU between process_samples and the policy update
-        self._pending = (itr, ops.PendingHost(b.sums), ops.PendingHost(b.maxs), ops.PendingHost(b.log_std))
+        if b.categorical:
+            # Entropy = mean over the valid samples of the state-dependent entropy(prob) (base.py:93)
+            ent = self._ent_buf(b)
+            ops.categorical_entropy(b, ent)
+            self.comm.all_reduce_mixed(ent, 2)
+            p_ent = ops.PendingHost(ent)
+        else:
+            p_ent = ops.PendingHost(b.log_std)
+        self._pending = (itr, ops.PendingHost(b.sums), ops.PendingHost(b.maxs), p_ent, b.categorical)
         self._stats = None
         for k in ("Iteration", "AverageDiscountedReturn", "AverageReturn", "ExplainedVariance", "NumTrajs", "Entropy",
                   "Perplexity", "StdReturn", "MaxReturn", "MinReturn"):
             logger.record_tabular(k, lambda k=k: self.stats[k])
         return samples_data
+
+    def _ent_buf(self, b):
+        import torch
+        buf = getattr(self, "_ent", None)
+        if buf is None or buf.device != b.device:
+            buf = self._ent = torch.zeros(2, dtype=torch.float64, device=b.device)
+        return buf
 
     @property
     def stats(self):
@@ -245,7 +267,8 @@ class LaneSampler(Sampler):
         return self._stats
 
     @staticmethod
-    def _resolve_stats(itr, p_sums, p_maxs, p_log_std):
+    def _resolve_stats(itr, p_sums, p_maxs, p_ent, categorical=False):
+        """p_ent: the categorical (entropy sum, sample count) when `categorical`, else the device log_std."""
         s, m = p_sums.get(), p_maxs.get()
         n_paths = s[3]
         avg_ret = s[5] / n_paths
@@ -256,7 +279,11 @@ class LaneSampler(Sampler):
             ev = 0 if varpred > 0 else 1
         else:
             ev = 1 - varres / (vary + 1e-8)
-        ent = float(np.sum(p_log_std.get().astype(np.float64) + np.log(np.sqrt(2 * np.pi * np.e))))
+        e = p_ent.get()
+        if categorical:
+            ent = float(e[0] / e[1])
+        else:
+            ent = float(np.sum(e.astype(np.float64) + np.log(np.sqrt(2 * np.pi * np.e))))
         return dict(
             Iteration=itr, AverageDiscountedReturn=s[4] / n_paths, AverageReturn=avg_ret, ExplainedVariance=ev,
             NumTrajs=int(round(n_paths)), Entropy=ent, Perplexity=np.exp(ent),

@@ -1,1 +1,2 @@
 from .box import Box  # noqa: F401
+from .discrete import Discrete  # noqa: F401
