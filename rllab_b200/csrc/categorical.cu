@@ -117,6 +117,73 @@ __device__ __forceinline__ void cat_terms(int loss_kind, const float (&p)[NA], c
   }
 }
 
+// Logit-space derivatives, float32 and float64, without differences of nearly equal numbers.  Softmax is shift-invariant,
+// so each is a sum over pairs (k, j) of a term symmetric in (k, j) times a difference of the pair: 1 - p_a is never
+// formed (it loses all accuracy in float32 once p_a rounds to 1, a logit gap of ~17), every product of probabilities
+// keeps the relative accuracy of its factors, and each row sums to zero bit for bit (at n = 2, dz_1 = -dz_0 exactly),
+// as the exact derivatives do.  The operations are rounded one by one so that the pair terms are computed alike.
+__device__ __forceinline__ float cat_mul(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ float cat_add(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ float cat_sub(float a, float b) { return __fsub_rn(a, b); }
+__device__ __forceinline__ double cat_mul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double cat_add(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double cat_sub(double a, double b) { return __dsub_rn(a, b); }
+
+// d term / dz_k = -c p_k (x_k - pa) = c sum_{j != k} (p_k p_j) (x_j - x_k)   (x one-hot, pa = sum_j p_j x_j)
+template <int NA, class T>
+__device__ __forceinline__ void cat_surr_logit_grad(T c, const T (&p)[NA], const T (&x)[NA], T (&dz)[NA]) {
+#pragma unroll
+  for (int k = 0; k < NA; ++k) {
+    T d = T(0);
+#pragma unroll
+    for (int j = 0; j < NA; ++j)
+      if (j != k) d = cat_add(d, cat_mul(cat_mul(p[k], p[j]), cat_sub(x[j], x[k])));
+    dz[k] = cat_mul(c, d);
+  }
+}
+
+// d kl(q || softmax(z)) / dz_k = -r_k + p_k sum_j r_j = sum_{j != k} (p_k r_j - r_k p_j),   r_j = q_j p_j / (p_j + TINY)
+template <int NA, class T>
+__device__ __forceinline__ void cat_kl_logit_grad(const T (&p)[NA], const T (&r)[NA], T (&g)[NA]) {
+#pragma unroll
+  for (int k = 0; k < NA; ++k) {
+    T d = T(0);
+#pragma unroll
+    for (int j = 0; j < NA; ++j)
+      if (j != k) d = cat_add(d, cat_sub(cat_mul(p[k], r[j]), cat_mul(r[k], p[j])));
+    g[k] = d;
+  }
+}
+
+// M tz, M = diag(R p - s) + s p^T + p s^T - (R + S) p p^T (the Hessian of kl(q || softmax(z)) in z at q = p; R = sum
+// p_j^2 / (p_j + TINY), s_j = TINY p_j^2 / (p_j + TINY)^2, S = sum s_j).  M's rows sum to zero, so
+//   (M tz)_k = sum_{j != k} W_kj (tz_k - tz_j),   W_kj = -M_kj = (R + S) p_k p_j - (s_k p_j + s_j p_k),
+// and W_kj loses at most a quarter to cancellation (s_j <= p_j / 4).
+template <int NA, class T>
+__device__ __forceinline__ void cat_logit_hvp(const T (&p)[NA], const T (&tz)[NA], T (&m)[NA]) {
+  constexpr T E = T(1e-8);   // TINY, exact in each type (float32: CAT_TINY)
+  T s[NA], R = T(0), S = T(0);
+#pragma unroll
+  for (int k = 0; k < NA; ++k) {
+    const T pe = p[k] + E;
+    R += p[k] * p[k] / pe;
+    s[k] = E * p[k] * p[k] / (pe * pe);
+    S += s[k];
+  }
+  const T RS = cat_add(R, S);
+#pragma unroll
+  for (int k = 0; k < NA; ++k) {
+    T d = T(0);
+#pragma unroll
+    for (int j = 0; j < NA; ++j) {
+      if (j == k) continue;
+      const T w = cat_sub(cat_mul(RS, cat_mul(p[k], p[j])), cat_add(cat_mul(s[k], p[j]), cat_mul(s[j], p[k])));
+      d = cat_add(d, cat_mul(w, cat_sub(tz[k], tz[j])));
+    }
+    m[k] = d;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ rollout / get_actions
 struct CatRolloutArgs {
   const float* params;
@@ -335,18 +402,14 @@ __device__ __forceinline__ void cat_phase_a(const UpdArgs& a, const float* sp, c
       if (!valid) { c = 0.f; term = 0.f; }
       s_loss += (double)term;
       if (valid) { s_kl += (double)kl; m_kl = fmax(m_kl, (double)kl); }
-#pragma unroll
-      for (int k = 0; k < A; ++k) dz[k] = -c * p[k] * (xa[k] - pa);
+      cat_surr_logit_grad(c, p, xa, dz);
       if (MODE == MODE_GRAD_KL && valid) {
-        // d kl / dz_j = -r_j + p_j sum_k r_k,  r_k = q_k p_k / (p_k + TINY)
-        float r[A], rs = 0.f;
+        float r[A], g[A];
 #pragma unroll
-        for (int k = 0; k < A; ++k) {
-          r[k] = q[k] * p[k] / (p[k] + CAT_TINY);
-          rs += r[k];
-        }
+        for (int k = 0; k < A; ++k) r[k] = q[k] * p[k] / (p[k] + CAT_TINY);
+        cat_kl_logit_grad(p, r, g);
 #pragma unroll
-        for (int k = 0; k < A; ++k) dz[k] = fmaf(a.penalty, fmaf(p[k], rs, -r[k]), dz[k]);
+        for (int k = 0; k < A; ++k) dz[k] = fmaf(a.penalty, g[k], dz[k]);
       }
     } else {
       // tangent forward J x (x = sv): t1 = (1-h1^2)(x V0 + vb0); t2 = (1-h2^2)(t1 W1 + h1 V1 + vb1); tz = t2 Wout + h2 Vout + vbout
@@ -367,23 +430,11 @@ __device__ __forceinline__ void cat_phase_a(const UpdArgs& a, const float* sp, c
 #pragma unroll
         for (int k = 0; k < A; ++k) tz[k] = fmaf(t2j, sp[N::oWo + j * A + k], fmaf(h2j, sv[N::oWo + j * A + k], tz[k]));
       }
-      // M tz, M = Hessian of kl(q || softmax(z)) in z at q = p (DESIGN.md section 5):
-      //   M = diag(R p - s) + s p^T + p s^T - (R + S) p p^T,  R = sum p_k^2 / (p_k + e),  s_k = e p_k^2 / (p_k + e)^2,  S = sum s_k
-      float s_[A], R = 0.f, S = 0.f, ptz = 0.f, stz = 0.f;
+      // M tz, M = Hessian of kl(q || softmax(z)) in z at q = p (DESIGN.md section 5)
+      float m[A];
+      cat_logit_hvp(p, tz, m);
 #pragma unroll
-      for (int k = 0; k < A; ++k) {
-        const float pe = p[k] + CAT_TINY;
-        R += p[k] * p[k] / pe;
-        s_[k] = CAT_TINY * p[k] * p[k] / (pe * pe);
-        S += s_[k];
-        ptz = fmaf(p[k], tz[k], ptz);
-        stz = fmaf(s_[k], tz[k], stz);
-      }
-#pragma unroll
-      for (int k = 0; k < A; ++k) {
-        const float m = (R * p[k] - s_[k]) * tz[k] + s_[k] * ptz + p[k] * stz - (R + S) * p[k] * ptz;
-        dz[k] = valid ? m : 0.f;
-      }
+      for (int k = 0; k < A; ++k) dz[k] = valid ? m[k] : 0.f;
     }
 #pragma unroll
     for (int k = 0; k < A; ++k) {
@@ -580,7 +631,7 @@ __global__ void __launch_bounds__(128) cat_f64_kernel(CatArgs64 a) {
     // FVP: tangent (J x) and the extra operands of the curvature term
     double th1[H], th2[H], g[A];
     if (MODE != MODE_FVP) {
-      double xa[A], q[A], pa = 0.0, qa = 0.0, kl = 0.0, r[A], rs = 0.0;
+      double xa[A], q[A], pa = 0.0, qa = 0.0, kl = 0.0, r[A];
 #pragma unroll
       for (int k = 0; k < A; ++k) {
         xa[k] = (double)a.act[(size_t)k * a.B + s];
@@ -589,7 +640,6 @@ __global__ void __launch_bounds__(128) cat_f64_kernel(CatArgs64 a) {
         qa += q[k] * xa[k];
         kl += q[k] * (log(q[k] + E) - log(p[k] + E));
         r[k] = q[k] * p[k] / (p[k] + E);
-        rs += r[k];
       }
       const double adv_s = (double)a.adv[s];
       double term, c;
@@ -604,9 +654,10 @@ __global__ void __launch_bounds__(128) cat_f64_kernel(CatArgs64 a) {
       s_kl += kl;
       m_kl = fmax(m_kl, kl);
       if (MODE == MODE_LOSS) continue;
-#pragma unroll
-      for (int k = 0; k < A; ++k)
-        dz[k] = (a.loss_kind == B200RL_LOSS_KL) ? (-r[k] + p[k] * rs) : (-c * p[k] * (xa[k] - pa));
+      if (a.loss_kind == B200RL_LOSS_KL)
+        cat_kl_logit_grad(p, r, dz);
+      else
+        cat_surr_logit_grad(c, p, xa, dz);
     } else {
       cat_dense_d<O, H>(sv + N::oW0, sv + N::ob0, x, th1);
 #pragma unroll
@@ -627,22 +678,11 @@ __global__ void __launch_bounds__(128) cat_f64_kernel(CatArgs64 a) {
         tz[k] = m;
       }
       // M tz (q = p) and g = d kl / dz at q = p
-      double s_[A], R = 0.0, S = 0.0, ptz = 0.0, stz = 0.0, r[A];
+      double r[A];
 #pragma unroll
-      for (int k = 0; k < A; ++k) {
-        const double pe = p[k] + E;
-        r[k] = p[k] * p[k] / pe;
-        R += r[k];
-        s_[k] = E * p[k] * p[k] / (pe * pe);
-        S += s_[k];
-        ptz += p[k] * tz[k];
-        stz += s_[k] * tz[k];
-      }
-#pragma unroll
-      for (int k = 0; k < A; ++k) {
-        dz[k] = (R * p[k] - s_[k]) * tz[k] + s_[k] * ptz + p[k] * stz - (R + S) * p[k] * ptz;
-        g[k] = -r[k] + p[k] * R;
-      }
+      for (int k = 0; k < A; ++k) r[k] = p[k] * p[k] / (p[k] + E);
+      cat_logit_hvp(p, tz, dz);
+      cat_kl_logit_grad(p, r, g);
     }
     // backward + accumulation.  FVP adds the tangent of g's backward pass:
     //   dWout += th2 (x) g;  D2 = d2(dz) + (g Vout^T)(1-h2^2) - 2 (g Wout^T) h2 th2;  dW1 += h1 (x) D2 + th1 (x) d2(g);

@@ -63,6 +63,16 @@ def prob(flat, obs, dims):
     return softmax(forward(flat, obs, dims)[0])
 
 
+def saturated_params(dims, gap, rng, sign=1.0):
+    """theta (n = 2) whose logit gap z0 - z1 lies within gap +- 0.25 at every input (sign -1: z1 - z0): Wout scaled so
+    that |h2 (Wout[:, 0] - Wout[:, 1])| <= 0.25 for any |h2| <= 1, bout = +-gap / 2; non-zero hidden biases."""
+    assert dims.A == 2
+    ts = unpack(init_params(dims, rng) + 0.05 * rng.randn(dims.P), dims)
+    ts[-2] *= 0.25 / np.abs(ts[-2][:, 0] - ts[-2][:, 1]).sum()
+    ts[-1] = sign * 0.5 * gap * np.array([1.0, -1.0])
+    return np.concatenate([t.reshape(-1) for t in ts])
+
+
 def weighted_sample_n(p, u):
     """special.weighted_sample_n with the uniforms given: #{k : cumsum_k(p) < u}, clipped to n - 1."""
     k = (np.cumsum(p, axis=1) < np.asarray(u).reshape(-1, 1)).sum(axis=1)
@@ -112,37 +122,80 @@ def _backward(flat, dims, acts, dz):
     return np.concatenate([g.reshape(-1) for g in grads])
 
 
+# The logit-space terms below are written without differences of nearly equal numbers, so that they stay exact when
+# one probability is near 1 (a confident policy).  Softmax is shift-invariant, so wherever the textbook form has
+# 1 - p_a or y_k - sum_j p_j y_j, it is computed as sum_j p_j (y_k - y_j): each p_j is accurate to rounding relative to
+# itself, and the terms of the sum are exact differences of the y's.  (The direct forms lose all accuracy in float64
+# once the smaller probability falls below ~1e-16 of the larger, a logit gap of ~37.)
+def _centered(p, y):
+    """y_k - sum_j p_j y_j as sum_j p_j (y_k - y_j), (B, n)."""
+    return np.einsum("bj,bkj->bk", p, y[:, :, None] - y[:, None, :])
+
+
+def _kl_logit_grad(p, q):
+    """d kl(q || softmax(z)) / dz_k = -r_k + p_k sum_j r_j, r = q p / (p + TINY), as sum_j (p_k r_j - r_k p_j)."""
+    r = q * p / (p + TINY)
+    return np.sum(p[:, :, None] * r[:, None, :] - r[:, :, None] * p[:, None, :], axis=2)
+
+
+def logit_grad(p, batch, kind, penalty=0.0):
+    """d (surrogate term + penalty kl) / dz per sample (B, n): -c p_k (x_k - pa) with x_k - pa = sum_j p_j (x_k - x_j)."""
+    x, q, adv = batch["actions"], batch["old_prob"], batch["adv"]
+    pa = np.sum(p * x, axis=-1)
+    c = adv / (np.sum(q * x, axis=-1) + TINY) if kind == "trpo" else adv / (pa + TINY)
+    dz = -c[:, None] * p * _centered(p, x)
+    if penalty:
+        dz = dz + penalty * _kl_logit_grad(p, q)
+    return dz
+
+
 def grad_surr(flat, batch, dims, kind, penalty=0.0):
     """Flat gradient of the surrogate + penalty * mean KL(old || new) (the objective of PPO's penalised step)."""
     z, acts = forward(flat, batch["obs"], dims)
-    p = softmax(z)
-    x, q, adv = batch["actions"], batch["old_prob"], batch["adv"]
-    B = p.shape[0]
-    pa = np.sum(p * x, axis=-1)
-    c = adv / (np.sum(q * x, axis=-1) + TINY) if kind == "trpo" else adv / (pa + TINY)
-    dz = -c[:, None] * p * (x - pa[:, None])
-    if penalty:
-        r = q * p / (p + TINY)
-        dz = dz + penalty * (-r + p * r.sum(axis=-1, keepdims=True))
-    return _backward(flat, dims, acts, dz / B)
+    dz = logit_grad(softmax(z), batch, kind, penalty)
+    return _backward(flat, dims, acts, dz / dz.shape[0])
 
 
-def logit_hessian(p):
-    """Hessian in z of kl(q || softmax(z)) at q = softmax(z), TINY kept (B, n, n)."""
+def grad_kl(flat, batch, dims):
+    """Flat gradient of mean KL(old || new) (FiniteDifferenceHvp's gradient, b200rl_categorical_update_f64's LOSS_KL)."""
+    z, acts = forward(flat, batch["obs"], dims)
+    g = _kl_logit_grad(softmax(z), batch["old_prob"])
+    return _backward(flat, dims, acts, g / g.shape[0])
+
+
+def _hessian_terms(p):
     pe = p + TINY
     R = np.sum(p * p / pe, axis=-1)
     s = TINY * p * p / (pe * pe)
+    return R, s
+
+
+def logit_hessian(p):
+    """Hessian in z of kl(q || softmax(z)) at q = softmax(z), TINY kept (B, n, n):
+    M = diag(R p - s) + s p^T + p s^T - (R + S) p p^T.  Its rows sum to zero (shift invariance), so the diagonal is
+    minus the sum of the off-diagonal entries, which have no cancellation."""
+    R, s = _hessian_terms(p)
     S = s.sum(axis=-1)
-    M = (R[:, None] * p - s)[:, :, None] * np.eye(p.shape[1])[None]
-    M += s[:, :, None] * p[:, None, :] + p[:, :, None] * s[:, None, :]
+    M = s[:, :, None] * p[:, None, :] + p[:, :, None] * s[:, None, :]
     M -= (R + S)[:, None, None] * p[:, :, None] * p[:, None, :]
+    n = p.shape[1]
+    M[:, np.arange(n), np.arange(n)] = 0.0
+    M[:, np.arange(n), np.arange(n)] = -M.sum(axis=2)
     return M
 
 
-def fvp(flat, batch, x, dims, reg_coeff=1e-5):
+def logit_hvp(p, tz):
+    """M tz per sample (B, n) as (R p_k - s_k) u_k + p_k sum_j s_j u_j, u = tz - p.tz = sum_j p_j (tz_k - tz_j)."""
+    R, s = _hessian_terms(p)
+    u = _centered(p, tz)
+    return (R[:, None] * p - s) * u + p * np.sum(s * u, axis=-1, keepdims=True)
+
+
+def fvp(flat, batch, x, dims, reg_coeff=1e-5, curvature=True):
     """Hx = grad(grad(mean KL) . x) + reg * x at theta_old (PerlmutterHvp, conjugate_gradient_optimizer.py:22-55), exact
     in float64: J^T M J x / B plus sum_j g_j (d^2 z_j)[x] / B, g = d kl / dz (O(TINY) at theta_old, DESIGN.md section 5),
-    the second term as the tangent along x of the backward pass of g."""
+    the second term as the tangent along x of the backward pass of g.  curvature=False leaves the second term out: the
+    Gauss-Newton product J^T M J x / B of the float32 pass (b200rl_categorical_fvp)."""
     ts, xs = unpack(flat, dims), unpack(x, dims)
     assert len(dims.H) == 2
     W0, b0, W1, b1, Wo, bo = ts
@@ -154,9 +207,8 @@ def fvp(flat, batch, x, dims, reg_coeff=1e-5):
     t1 = d1h * (X @ V0 + c0)
     t2 = d2h * (t1 @ W1 + h1 @ V1 + c1)
     tz = t2 @ Wo + h2 @ Vo + co
-    dz = np.einsum("bij,bj->bi", logit_hessian(p), tz)
-    r = p * p / (p + TINY)
-    g = -r + p * r.sum(axis=-1, keepdims=True)
+    dz = logit_hvp(p, tz)
+    g = _kl_logit_grad(p, p) if curvature else np.zeros_like(p)
     d2g = (g @ Wo.T) * d2h
     D2 = (dz @ Wo.T) * d2h + (g @ Vo.T) * d2h - 2.0 * (g @ Wo.T) * h2 * t2
     D1 = (D2 @ W1.T + d2g @ V1.T) * d1h - 2.0 * (d2g @ W1.T) * h1 * t1
@@ -164,11 +216,12 @@ def fvp(flat, batch, x, dims, reg_coeff=1e-5):
     return np.concatenate([o.reshape(-1) for o in out]) / B + reg_coeff * np.asarray(x)
 
 
-def trpo_step(theta, batch, dims, step_size=0.01, cg_iters=10, reg_coeff=1e-5):
+def trpo_step(theta, batch, dims, step_size=0.01, cg_iters=10, reg_coeff=1e-5, curvature=True):
+    """One TRPO step; curvature=False solves with the Gauss-Newton product of the float32 pass (see fvp)."""
     f_loss = lambda th: surr_loss(th, batch, dims, "trpo")
     f_grad = lambda th: grad_surr(th, batch, dims, "trpo")
     f_lc = lambda th: (surr_loss(th, batch, dims, "trpo"), kl_stats(th, batch, dims)[0])
-    f_Hx = lambda th, v: fvp(th, batch, v, dims, reg_coeff)
+    f_Hx = lambda th, v: fvp(th, batch, v, dims, reg_coeff, curvature)
     return OPT.trpo_optimize(f_loss, f_grad, f_lc, f_Hx, theta, step_size, cg_iters)
 
 

@@ -92,6 +92,108 @@ def test_oracle_ratio_one_and_kl_zero_at_theta_old():
     assert C.kl_stats(theta, batch, DIMS) == (0.0, 0.0)
 
 
+GAPS = (4, 8, 12, 16, 20, 30, 60)          # logit gaps |z0 - z1| of the saturated buckets
+
+
+def _mp_reference(theta, batch, x, kind, penalty):
+    """(surrogate + penalty KL gradient, KL gradient, Fisher-vector product at theta_old = theta with q = p) in 50-digit
+    arithmetic, by the textbook formulas (dz = -c p (x - pa), M = diag(R p - s) + s p^T + p s^T - (R + S) p p^T): at
+    this precision their cancellation costs nothing."""
+    mp = pytest.importorskip("mpmath")
+    with mp.workdps(50):
+        f = np.vectorize(lambda v: mp.mpf(float(v)), otypes=[object])
+        tanh = np.vectorize(mp.tanh, otypes=[object])
+        exp = np.vectorize(mp.exp, otypes=[object])
+        E = mp.mpf(C.TINY)
+        W0, b0, W1, b1, Wo, bo = (f(t) for t in C.unpack(theta, DIMS))
+        V0, c0, V1, c1, Vo, co = (f(t) for t in C.unpack(x, DIMS))
+        X, xa, q, adv = (f(batch[k]) for k in ("obs", "actions", "old_prob", "adv"))
+        B = X.shape[0]
+        h1 = tanh(X @ W0 + b0)
+        h2 = tanh(h1 @ W1 + b1)
+        z = h2 @ Wo + bo
+        e = exp(z - np.max(z, axis=1, keepdims=True))
+        p = e / np.sum(e, axis=1, keepdims=True)
+
+        def backward(dz):
+            d2 = (dz @ Wo.T) * (1 - h2 * h2)
+            d1 = (d2 @ W1.T) * (1 - h1 * h1)
+            return np.concatenate([(X.T @ d1).reshape(-1), d1.sum(0), (h1.T @ d2).reshape(-1), d2.sum(0),
+                                   (h2.T @ dz).reshape(-1), dz.sum(0)]) / B
+
+        pa = np.sum(p * xa, axis=1)
+        c = adv / (np.sum(q * xa, axis=1) + E) if kind == "trpo" else adv / (pa + E)
+        r = q * p / (p + E)
+        gkl = -r + p * np.sum(r, axis=1, keepdims=True)
+        g = backward(-c[:, None] * p * (xa - pa[:, None]) + penalty * gkl)
+        g_kl = backward(gkl)
+        # Fisher-vector product at q = p: J^T M J x + sum_j g_j (d^2 z_j)[x], as tests/categorical_oracle.py:fvp
+        d1h, d2h = 1 - h1 * h1, 1 - h2 * h2
+        t1 = d1h * (X @ V0 + c0)
+        t2 = d2h * (t1 @ W1 + h1 @ V1 + c1)
+        tz = t2 @ Wo + h2 @ Vo + co
+        pe = p + E
+        R = np.sum(p * p / pe, axis=1)[:, None]
+        s = E * p * p / (pe * pe)
+        S = np.sum(s, axis=1)[:, None]
+        ptz = np.sum(p * tz, axis=1)[:, None]
+        stz = np.sum(s * tz, axis=1)[:, None]
+        mz = (R * p - s) * tz + s * ptz + p * stz - (R + S) * p * ptz
+        rr = p * p / pe
+        gg = -rr + p * np.sum(rr, axis=1, keepdims=True)
+        d2g = (gg @ Wo.T) * d2h
+        D2 = (mz @ Wo.T) * d2h + (gg @ Vo.T) * d2h - 2 * (gg @ Wo.T) * h2 * t2
+        D1 = (D2 @ W1.T + d2g @ V1.T) * d1h - 2 * (d2g @ W1.T) * h1 * t1
+        hx = np.concatenate([(X.T @ D1).reshape(-1), D1.sum(0), (h1.T @ D2 + t1.T @ d2g).reshape(-1), D2.sum(0),
+                             (h2.T @ mz + t2.T @ gg).reshape(-1), mz.sum(0)]) / B
+        return tuple(np.array([float(v) for v in a]) for a in (g, g_kl, hx))
+
+
+def _blocks():
+    out, k = [], 0
+    for s in DIMS.shapes:
+        n = int(np.prod(s))
+        out.append(slice(k, k + n))
+        k += n
+    return out
+
+
+def saturated_batch(rng, gap, sign, B=8, n_unlikely=2):
+    """A batch at theta_old = C.saturated_params(gap): actions drawn from the policy, the last n_unlikely forced to the
+    unlikely action (q down to its probability, 1e-26 at gap 60)."""
+    theta = C.saturated_params(DIMS, gap, rng, sign)
+    obs = rng.randn(B, 4)
+    p = C.prob(theta, obs, DIMS)
+    acts = C.weighted_sample_n(p, rng.rand(B))
+    acts[B - n_unlikely:] = np.argmin(p[B - n_unlikely:], axis=1)
+    return dict(obs=obs, actions=np.eye(2)[acts], adv=rng.randn(B), old_prob=p), theta
+
+
+@pytest.mark.parametrize("gap", GAPS)
+def test_oracle_exact_at_saturated_softmax(gap):
+    """The oracle's gradients (TRPO and VPG surrogates, with and without a KL penalty, off theta_old), KL gradient and
+    Fisher-vector product (at theta_old, TINY terms included) within 1e-13 of 50-digit arithmetic, per parameter block,
+    on a batch whose every logit gap is `gap`: no term of it may cancel when a probability nears 1."""
+    rng = np.random.RandomState(gap)
+    batch, theta_old = saturated_batch(rng, gap, 1.0 if gap % 8 else -1.0)
+    p = C.prob(theta_old, batch["obs"], DIMS)
+    assert np.all(np.abs(np.log(p[:, 0]) - np.log(p[:, 1])) > gap - 0.3)
+    theta = theta_old + 0.01 * rng.randn(DIMS.P)
+    x = rng.randn(DIMS.P)
+    checks = []
+    for kind, pen in (("trpo", 0.0), ("trpo", 2.5), ("vpg", 0.0), ("vpg", 2.5)):
+        g_ref, gkl_ref, _ = _mp_reference(theta, batch, x, kind, pen)
+        checks.append(("grad %s pen %g" % (kind, pen), C.grad_surr(theta, batch, DIMS, kind, pen), g_ref))
+    checks.append(("kl grad", C.grad_kl(theta, batch, DIMS), gkl_ref))
+    batch_old = dict(batch, old_prob=p)
+    _, _, hx_ref = _mp_reference(theta_old, batch_old, x, "trpo", 0.0)
+    checks.append(("fvp", C.fvp(theta_old, batch_old, x, DIMS, reg_coeff=0.0), hx_ref))
+    for what, got, ref in checks:
+        for i, sl in enumerate(_blocks()):
+            err = np.abs(got[sl] - ref[sl]).max() / np.abs(ref[sl]).max()
+            assert err <= 1e-13, "gap %g, %s, block %d: %.3g" % (gap, what, i, err)
+
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_categorical_golden.npz")
 
 

@@ -1,11 +1,13 @@
-"""The GPU grids that claim to cover every env kind name exactly the kinds of rllab_b200._lib.ENV_KINDS, so that a new
-env kind cannot skip them unnoticed.  No GPU needed: the grids are module constants."""
+"""The GPU grids that claim to cover every env kind name exactly the kinds of rllab_b200._lib.ENV_KINDS (the discrete
+grids: DISCRETE_ENV_KINDS), so that a new env kind cannot skip them unnoticed.  No GPU needed: the grids are module
+constants."""
 import pytest
 
 pytest.importorskip("torch")
 
 from rllab_b200 import _lib as L        # noqa: E402
 import test_gpu_algos                   # noqa: E402
+import test_gpu_categorical_shapes      # noqa: E402
 import test_gpu_cem                     # noqa: E402
 import test_gpu_process_shapes          # noqa: E402
 import test_gpu_rollout_shapes          # noqa: E402
@@ -25,11 +27,24 @@ GRIDS = {
     "planar_episodes": lambda: [e for e, _ in test_gpu_round2.PLANAR_EPISODES],
 }
 
+# grids over the discrete-action kinds (rllab_b200._lib.DISCRETE_ENV_KINDS)
+DISCRETE_GRIDS = {
+    "discrete_rollout": lambda: test_gpu_categorical_shapes.DISCRETE_ENVS,
+}
+
 
 @pytest.mark.parametrize("grid", sorted(GRIDS))
 def test_grid_covers_every_env_kind(grid):
     names = set(GRIDS[grid]())
     expected = set(L.ENV_KINDS) - EXCLUDED.get(grid, set())
+    assert names == expected, "%s grid: missing %s, unknown %s" % (grid, sorted(expected - names),
+                                                                   sorted(names - expected))
+
+
+@pytest.mark.parametrize("grid", sorted(DISCRETE_GRIDS))
+def test_grid_covers_every_discrete_env_kind(grid):
+    names = set(DISCRETE_GRIDS[grid]())
+    expected = set(L.DISCRETE_ENV_KINDS)
     assert names == expected, "%s grid: missing %s, unknown %s" % (grid, sorted(expected - names),
                                                                    sorted(names - expected))
 
