@@ -298,6 +298,71 @@ int b200rl_categorical_update_f64(int mode, int loss_kind, const double* params_
 int b200rl_categorical_entropy(int n_actions, long long B, const float* prob, const unsigned char* flags, double* out,
                                double* ws, void* stream);
 
+/* ---- GaussianGRUPolicy (rllab/policies/gaussian_gru_policy.py, rllab/core/network.py:104-270 GRULayer / GRUNetwork,
+ * rllab/distributions/recurrent_diagonal_gaussian.py).  x_t = [obs_t, prev_action_t] (include_action != 0) or obs_t;
+ * r = sigma(x W_xr + h W_hr + b_r), u = sigma(x W_xu + h W_hu + b_u), c = tanh(x W_xc + r * (h W_hc) + b_c),
+ * h' = (1 - u) h + u c, mean = h' W_out + b_out, log_std a state-independent parameter (no min_std clamp).  h = 0 and
+ * prev_action = 0 at a path start (tstep == 0); inside a path prev_action is the previous raw action act[t-1].  Flat
+ * layout [W_xr (I x H), W_hr (H x H), b_r, W_xu, W_hu, b_u, W_xc, W_hc, b_c, W_out (H x A), b_out, log_std].  Compiled
+ * for obs_dim 4, hidden 32, act_dim 1 (CartpoleEnv), either include_action; other shapes return B200RL_EUNSUPPORTED.
+ * The update passes take the lane geometry (N lanes, T steps, B = N T samples, planes [.][T][N]) and tstep, from
+ * which they rebuild each lane's inputs and hidden states. ---- */
+
+/* Number of GRU policy parameters P (including log_std); <0 if the shape is not compiled in. */
+long long b200rl_gru_num_params(int obs_dim, int hidden, int act_dim, int include_action);
+
+/* One GRU step for n rows (GaussianGRUPolicy.get_action, vectorised): obs [O][n], prev_action [A][n] (NULL = 0), h_in
+ * [H][n] (NULL = 0) -> act_out = mean + exp(log_std) eps, mean_out [A][n], h_out [H][n], log_std_out [A].  eps [A][n]
+ * or NULL (Philox stream 0 at (lane0 + i, row), as b200rl_policy_get_actions). */
+int b200rl_gru_get_actions(const float* params_f32, int obs_dim, int hidden, int act_dim, int include_action,
+                           const float* obs, const float* prev_action, const float* h_in, long long n, const float* eps,
+                           unsigned int seed, unsigned int iter, int row, long long lane0, float* act_out,
+                           float* mean_out, float* h_out, float* log_std_out, void* stream);
+
+/* Fused rollout with the GRU policy: b200rl_rollout's lane semantics and planes (obs, raw act, mean, rew, flags, tstep,
+ * log_std_out), with h and prev_action carried per lane and reset at every path start. */
+int b200rl_rollout_gru(int env_kind, const float* params_f32, int hidden, int include_action, int N, int T,
+                       int max_path_length, const float* eps, const float* reset_raw, unsigned int seed,
+                       unsigned int iter, long long lane0, float* obs, float* act, float* mean, float* rew,
+                       unsigned char* flags, unsigned short* tstep, float* log_std_out, void* stream);
+
+/* (loss, sum KL, max KL) as b200rl_loss_kl over the lane batch (npo.py:67-82 with valids = not FLAG_MASKED);
+ * h_cache_out ([H][T][N] or NULL) receives h_t. */
+int b200rl_gru_loss_kl(int loss_kind, const float* params_f32, int obs_dim, int hidden, int act_dim,
+                       int include_action, int N, int T, const float* obs, const float* act,
+                       const unsigned short* tstep, const float* adv, const float* old_mean, const float* old_log_std,
+                       const unsigned char* flags, double scale, const double* count, double* out, float* h_cache_out,
+                       double* ws, void* stream);
+
+/* Backpropagation-through-time gradient of the surrogate plus penalty * mean KL (penalty 0: b200rl_grad, > 0:
+ * b200rl_grad_penalized); loss_out (3 or NULL) the unpenalised triple.  h_cache [H][T][N] is required: the forward sweep
+ * writes h_t there and the backward sweep reads it (a later b200rl_gru_fvp may reuse it with h_valid = 1). */
+int b200rl_gru_grad(int loss_kind, double penalty, const float* params_f32, int obs_dim, int hidden, int act_dim,
+                    int include_action, int N, int T, const float* obs, const float* act, const unsigned short* tstep,
+                    const float* adv, const float* old_mean, const float* old_log_std, const unsigned char* flags,
+                    double scale, const double* count, double* g_out, double* loss_out, float* h_cache, double* ws,
+                    void* stream);
+
+/* Fisher-vector product J^T M J x (+ diag_scale * reg_coeff * x, and the log_std block) at theta_old, as b200rl_fvp:
+ * a forward tangent sweep carries J x through h and writes M J x per sample into the workspace, then the gradient
+ * pass's backward sweep runs on those deltas.  h_cache [H][T][N] is required; h_valid != 0: it already holds h_t at
+ * these parameters (b200rl_gru_grad wrote it), else it is rewritten. */
+int b200rl_gru_fvp(const float* params_f32, int obs_dim, int hidden, int act_dim, int include_action, int N, int T,
+                   const float* obs, const float* act, const unsigned short* tstep, const unsigned char* flags,
+                   const double* x, double scale, const double* count, double reg_coeff, double diag_scale,
+                   double* Hx_out, float* h_cache, int h_valid, double* ws, void* stream);
+
+/* float64 parity mode of the passes above on the float64 master parameters, as b200rl_update_f64 (mode 0 loss/KL, 1
+ * gradient, 2 Fisher-vector product; loss_kind B200RL_LOSS_KL with mode 1 = gradient of mean KL for
+ * FiniteDifferenceHvp).  h64 [H + A][T][N] float64 scratch (hidden states, and M J x in mode 2).  Weight gradients are
+ * summed with float64 atomics: reruns agree to rounding. */
+int b200rl_gru_update_f64(int mode, int loss_kind, const double* params_f64, int obs_dim, int hidden, int act_dim,
+                          int include_action, int N, int T, const float* obs, const float* act,
+                          const unsigned short* tstep, const float* adv, const float* old_mean,
+                          const float* old_log_std, const unsigned char* flags, const double* x, double scale,
+                          const double* count, double reg_coeff, double diag_scale, double* vec_out, double* loss_out,
+                          double* h64, double* ws, void* stream);
+
 /* ---- GaussianMLPRegressor, the value function of GaussianMLPBaseline (rllab/regressors/gaussian_mlp_regressor.py,
  * rllab/baselines/gaussian_mlp_baseline.py).  Net: MLP(obs_dim -> h1 -> h2 -> 1), ReLU hidden units, no output
  * nonlinearity, one state-independent log_std (rllab/core/network.py:36-81, lasagne_layers.py ParamLayer); the flat

@@ -108,6 +108,19 @@ SIGNATURES = {
     "b200rl_categorical_entropy": (c_int, [c_int, _LL, _P, _P, _P, _P, _P]),
     "b200rl_categorical_update_f64": (c_int, [c_int, c_int, _P, c_int, c_int, c_int, c_int, _LL, _P, _P, _P, _P, _P,
                                               _P, c_double, _P, c_double, c_double, _P, _P, _P, _P]),
+    "b200rl_gru_num_params": (_LL, [c_int, c_int, c_int, c_int]),
+    "b200rl_gru_get_actions": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _LL, _P, c_uint, c_uint, c_int, _LL,
+                                       _P, _P, _P, _P, _P]),
+    "b200rl_rollout_gru": (c_int, [c_int, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_uint, c_uint, _LL, _P, _P,
+                                   _P, _P, _P, _P, _P, _P]),
+    "b200rl_gru_loss_kl": (c_int, [c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P,
+                                   c_double, _P, _P, _P, _P, _P]),
+    "b200rl_gru_grad": (c_int, [c_int, c_double, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P,
+                                _P, c_double, _P, _P, _P, _P, _P, _P]),
+    "b200rl_gru_fvp": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_double, _P, c_double,
+                               c_double, _P, _P, c_int, _P, _P]),
+    "b200rl_gru_update_f64": (c_int, [c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P,
+                                      _P, _P, _P, c_double, _P, c_double, c_double, _P, _P, _P, _P, _P]),
 }
 
 _lib = None
@@ -198,4 +211,11 @@ def categorical_num_params(O, h1, h2, n):
     p = load().b200rl_categorical_num_params(O, h1, h2, n)
     if p < 0:
         raise B200RLError("unsupported categorical network O=%d hidden=(%d,%d) n=%d: %s" % (O, h1, h2, n, last_error()))
+    return int(p)
+
+
+def gru_num_params(O, H, A, include_action):
+    p = load().b200rl_gru_num_params(O, H, A, int(bool(include_action)))
+    if p < 0:
+        raise B200RLError("unsupported GRU network O=%d hidden=%d A=%d: %s" % (O, H, A, last_error()))
     return int(p)

@@ -68,7 +68,7 @@ class CEM(RLAlgorithm, Serializable):
         if plot:
             raise NotImplementedError("plotting is outside the B200 hot path")
         from .. import ops
-        if ops.is_categorical(getattr(policy, "dims", None)):
+        if ops.is_categorical(getattr(policy, "dims", None)) or ops.is_gru(getattr(policy, "dims", None)):
             raise NotImplementedError("CEM's population rollout is built for GaussianMLPPolicy only")
         self.env = env
         self.policy = policy

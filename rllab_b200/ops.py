@@ -73,6 +73,8 @@ class LaneBatch(object):
         self.B_global = N * T         # samples over all ranks (the sampler overwrites it under torchrun)
         self.masked = False           # process_samples dropped cut paths: passes read FLAG_MASKED and the device count
         self.categorical = False      # act holds one-hot actions and mean the probabilities of a categorical policy
+        self.recurrent = False        # the batch was rolled out by a GRU policy (paths / samples_data: recurrent layout)
+        self.prev_action_info = False  # ... whose input includes the previous action (agent_infos["prev_action"])
 
     @property
     def B(self):
@@ -114,6 +116,59 @@ class CategoricalDims(tuple):
 
 def is_categorical(dims):
     return isinstance(dims, CategoricalDims)
+
+
+class GRUDims(tuple):
+    """(O, H, A, include_action) of a GaussianGRUPolicy (its fields are not the (O, h1, h2, A) of the MLP policies: every
+    GRU branch below unpacks them as `O, H, A, inc = dims`).  Handed to the update passes below, this type makes them run the
+    GRU kernels (b200rl_gru_*) over the batch's lanes: they rebuild each lane's inputs and hidden states from obs, act
+    and tstep.  batch.mean / batch.log_std hold the old mean and log_std, as for the Gaussian MLP policy."""
+
+    def __new__(cls, O, H, A, include_action):
+        return tuple.__new__(cls, (int(O), int(H), int(A), int(bool(include_action))))
+
+    def __getnewargs__(self):
+        return tuple(self)
+
+
+def is_gru(dims):
+    return isinstance(dims, GRUDims)
+
+
+def _gru_hbuf(batch, H):
+    """[H][T][N] float32 hidden states of the GRU passes: the batch's activation cache buffer."""
+    return batch.hcache(H, 0)
+
+
+def _gru_h64(batch, H, A):
+    """[H+A][T][N] float64 scratch of the GRU parity passes (allocated on first use)."""
+    h = getattr(batch, "_gru_h64", None)
+    if h is None or h.shape[0] != H + A:
+        h = torch.empty((H + A, batch.T, batch.N), dtype=F64, device=batch.device)
+        batch._gru_h64 = h
+    return h
+
+
+def gru_rollout(dims, params32, batch, max_path_length, kind, eps=None, reset_raw=None, seed=0, it=0, lane0=0):
+    """Fused rollout with the GRU policy (b200rl_rollout_gru): b200rl_rollout's planes, h and prev_action per lane."""
+    O, H, A, inc = dims
+    b = batch
+    _chk(params32, F32, "params32"), _chk(eps, F32, "eps"), _chk(reset_raw, F32, "reset_raw")
+    L.call("b200rl_rollout_gru", kind, L.ptr(params32), H, inc, b.N, b.T, max_path_length, L.ptr(eps), L.ptr(reset_raw),
+           seed, it, lane0, L.ptr(b.obs), L.ptr(b.act), L.ptr(b.mean), L.ptr(b.rew), L.ptr(b.flags), L.ptr(b.tstep),
+           L.ptr(b.log_std), _stream())
+
+
+def gru_get_actions(params32, dims, obs, prev_action, h_in, n, eps, seed, it, row, lane0, act_out, mean_out, h_out,
+                    log_std_out):
+    """One GRU step of n rows (b200rl_gru_get_actions); prev_action / h_in None = zeros."""
+    O, H, A, inc = dims
+    _chk(params32, F32, "params32"), _chk(obs, F32, "obs", O * n), _chk(prev_action, F32, "prev_action", A * n)
+    _chk(h_in, F32, "h_in", H * n), _chk(eps, F32, "eps", A * n), _chk(act_out, F32, "act_out", A * n)
+    _chk(mean_out, F32, "mean_out", A * n), _chk(h_out, F32, "h_out", H * n), _chk(log_std_out, F32, "log_std_out", A)
+    L.call("b200rl_gru_get_actions", L.ptr(params32), O, H, A, inc, L.ptr(obs), L.ptr(prev_action), L.ptr(h_in), n,
+           L.ptr(eps), seed, it, row, lane0, L.ptr(act_out), L.ptr(mean_out), L.ptr(h_out), L.ptr(log_std_out),
+           _stream())
 
 
 _n_actions = {}
@@ -291,6 +346,13 @@ def loss_kl(loss_kind, params32, dims, min_std, batch, out, fuse=False):
     b = batch
     fl, scale, cnt = _mask(b)
     _chk(params32, F32, "params32"), _chk(out, F64, "out", 3)
+    if is_gru(dims):
+        O, H, A, inc = dims
+        with _Fused(fuse):
+            L.call("b200rl_gru_loss_kl", loss_kind, L.ptr(params32), O, H, A, inc, b.N, b.T, L.ptr(b.obs), L.ptr(b.act),
+                   L.ptr(b.tstep), L.ptr(b.adv), L.ptr(b.mean), L.ptr(b.log_std), fl, scale, cnt, L.ptr(out), None,
+                   L.ptr(workspace(b.device)), _stream())
+        return
     if is_categorical(dims):
         with _Fused(fuse):
             L.call("b200rl_categorical_loss_kl", loss_kind, L.ptr(params32), O, h1, h2, A, b.B, L.ptr(b.obs),
@@ -308,6 +370,9 @@ def grad(loss_kind, params32, dims, min_std, batch, g_out, loss_out=None, h_cach
     b = batch
     fl, scale, cnt = _mask(b)
     _chk(params32, F32, "params32"), _chk(g_out, F64, "g_out")
+    if is_gru(dims):
+        _gru_grad(loss_kind, 0.0, params32, dims, b, g_out, loss_out, h_cache, fuse)
+        return
     if is_categorical(dims):
         _categorical_grad(loss_kind, 0.0, params32, dims, b, g_out, loss_out, h_cache, fuse)
         return
@@ -324,6 +389,9 @@ def grad_penalized(loss_kind, penalty, params32, dims, min_std, batch, g_out, lo
     b = batch
     fl, scale, cnt = _mask(b)
     _chk(params32, F32, "params32"), _chk(g_out, F64, "g_out")
+    if is_gru(dims):
+        _gru_grad(loss_kind, penalty, params32, dims, b, g_out, loss_out, None, fuse)
+        return
     if is_categorical(dims):
         _categorical_grad(loss_kind, penalty, params32, dims, b, g_out, loss_out, None, fuse)
         return
@@ -343,6 +411,19 @@ def _categorical_grad(loss_kind, penalty, params32, dims, batch, g_out, loss_out
                L.ptr(h_cache), L.ptr(workspace(b.device)), _stream())
 
 
+def _gru_grad(loss_kind, penalty, params32, dims, batch, g_out, loss_out, h_cache, fuse):
+    """The BPTT pass always writes h_t: into h_cache when given, else into the batch's own buffer."""
+    O, H, A, inc = dims
+    b = batch
+    fl, scale, cnt = _mask(b)
+    hb = h_cache if h_cache is not None else _gru_hbuf(b, H)
+    _chk(hb, F32, "h_cache", H * b.B)
+    with _Fused(fuse):
+        L.call("b200rl_gru_grad", loss_kind, float(penalty), L.ptr(params32), O, H, A, inc, b.N, b.T, L.ptr(b.obs),
+               L.ptr(b.act), L.ptr(b.tstep), L.ptr(b.adv), L.ptr(b.mean), L.ptr(b.log_std), fl, scale, cnt, L.ptr(g_out),
+               L.ptr(loss_out), L.ptr(hb), L.ptr(workspace(b.device)), _stream())
+
+
 def fvp(params32, dims, min_std, batch, x, reg_coeff, diag_scale, Hx_out, h_cache=None, tile_list=None, count=None,
         fuse=False):
     """tile_list (int32 device tensor) + count (float64 device scalar: valid samples in those tiles over all ranks):
@@ -353,6 +434,18 @@ def fvp(params32, dims, min_std, batch, x, reg_coeff, diag_scale, Hx_out, h_cach
     if tile_list is not None:
         scale, cnt = 1.0, L.ptr(count)
     _chk(params32, F32, "params32"), _chk(x, F64, "x"), _chk(Hx_out, F64, "Hx_out", x.numel())
+    if is_gru(dims):
+        if tile_list is not None:
+            raise NotImplementedError("sub-sampled Fisher products (subsample_factor < 1) are not built for the GRU "
+                                      "policy: the reference sub-samples whole paths, not tiles")
+        O, H, A, inc = dims
+        hb = h_cache if h_cache is not None else _gru_hbuf(b, H)
+        _chk(hb, F32, "h_cache", H * b.B)
+        with _Fused(fuse):
+            L.call("b200rl_gru_fvp", L.ptr(params32), O, H, A, inc, b.N, b.T, L.ptr(b.obs), L.ptr(b.act), L.ptr(b.tstep),
+                   fl, L.ptr(x), scale, cnt, float(reg_coeff), float(diag_scale), L.ptr(Hx_out), L.ptr(hb),
+                   int(h_cache is not None), L.ptr(workspace(b.device)), _stream())
+        return
     if is_categorical(dims):
         with _Fused(fuse):
             L.call("b200rl_categorical_fvp", L.ptr(params32), O, h1, h2, A, b.B, L.ptr(b.obs), fl, L.ptr(x), scale, cnt,
@@ -377,6 +470,14 @@ def update_f64(mode, loss_kind, params64, dims, min_std, batch, x, reg_coeff, di
     b = batch
     fl, scale, cnt = _mask(b)
     _chk(params64, F64, "params64"), _chk(x, F64, "x"), _chk(vec_out, F64, "vec_out"), _chk(loss_out, F64, "loss_out", 3)
+    if is_gru(dims):
+        O, H, A, inc = dims
+        with _Fused(fuse):
+            L.call("b200rl_gru_update_f64", mode, loss_kind, L.ptr(params64), O, H, A, inc, b.N, b.T, L.ptr(b.obs),
+                   L.ptr(b.act), L.ptr(b.tstep), L.ptr(b.adv), L.ptr(b.mean), L.ptr(b.log_std), fl, L.ptr(x), scale, cnt,
+                   float(reg_coeff), float(diag_scale), L.ptr(vec_out), L.ptr(loss_out), L.ptr(_gru_h64(b, H, A)),
+                   L.ptr(workspace(b.device)), _stream())
+        return
     if is_categorical(dims):
         with _Fused(fuse):
             L.call("b200rl_categorical_update_f64", mode, loss_kind, L.ptr(params64), O, h1, h2, A, b.B, L.ptr(b.obs),

@@ -225,6 +225,9 @@ class ConjugateGradientOptimizer(object):
         if self._subsample_factor < 1:
             if self._f64 or self._fd:
                 raise NotImplementedError("subsample_factor < 1 is built for the float32 Fisher-vector kernels")
+            if ops.is_gru(pol.dims):
+                raise NotImplementedError("subsample_factor < 1 is not built for a recurrent policy (the reference "
+                                          "sub-samples whole paths, not 128-sample tiles)")
             tiles = self._draw_subsample(batch, b)
 
         logger.log("computing loss before")

@@ -55,7 +55,8 @@ def lanes_to_paths(batch, whole_paths=True):
     """Device lanes -> list of path dicts {observations (L,O), actions (L,A), rewards (L,), agent_infos{mean,log_std},
     env_infos{}} (+ advantages / returns when process_samples has run), lane-major then time order.  whole_paths: leave
     out the paths cut by the end of the lane buffer (FLAG_CUT on their last sample).  A categorical batch has one-hot
-    actions (L,n) and agent_infos{prob}."""
+    actions (L,n) and agent_infos{prob}; a recurrent batch whose policy reads the previous action also carries
+    agent_infos["prev_action"] (zeros at the first step, then the path's previous raw action)."""
     t = batch.to_numpy()
     O, T, N = t["obs"].shape
     A = t["act"].shape[0]
@@ -79,6 +80,9 @@ def lanes_to_paths(batch, whole_paths=True):
                              dict(mean=t["mean"][:, sl, n].T.astype(np.float64), log_std=np.tile(ls, (e + 1 - start, 1)))),
                 env_infos=dict(),
             )
+            if getattr(batch, "prev_action_info", False):
+                a = p["actions"]
+                p["agent_infos"]["prev_action"] = np.concatenate([np.zeros((1, A)), a[:-1]], axis=0)
             if adv is not None:
                 p["advantages"] = adv[sl, n].astype(np.float64)
                 p["returns"] = ret[sl, n].astype(np.float64)
@@ -87,21 +91,54 @@ def lanes_to_paths(batch, whole_paths=True):
     return paths
 
 
+def recurrent_samples_entry(paths, key):
+    """Entry `key` of the reference's recurrent samples_data (sampler/base.py:105-161) from path dicts whose advantages
+    are already centred: every per-sample array zero-padded to (n_paths, max_path_len, ...) in path order, "valids" 1 on
+    the samples of each path, agent_infos padded key by key, env_infos empty."""
+    if key == "paths":
+        return paths
+    T = max(len(p["rewards"]) for p in paths)
+
+    def pad(x):
+        x = np.asarray(x)
+        out = np.zeros((T,) + x.shape[1:])
+        out[:len(x)] = x
+        return out
+    if key == "valids":
+        return np.asarray([pad(np.ones(len(p["rewards"]))) for p in paths])
+    if key == "agent_infos":
+        return {k: np.asarray([pad(p["agent_infos"][k]) for p in paths]) for k in paths[0]["agent_infos"]}
+    if key == "env_infos":
+        return dict()
+    return np.asarray([pad(p[key]) for p in paths])
+
+
 class SamplesData(dict):
     """samples_data of rllab/sampler/base.py:95-104.  The device batch is under "lane_batch"; the reference's host
     arrays ("observations", "actions", "rewards", "returns", "advantages", "agent_infos", "env_infos", "paths") are
-    materialised in the reference layout ((B, dim) float64, sample order t-major then lane) on first access."""
-    _LAZY = ("observations", "actions", "rewards", "returns", "advantages", "agent_infos", "env_infos", "paths")
+    materialised in the reference layout ((B, dim) float64, sample order t-major then lane) on first access.  For a
+    recurrent policy the layout is the reference's recurrent one (base.py:105-161): every array padded with zeros to
+    (n_paths, max_path_len, ...) in path order, plus "valids" (1 on the samples of each path)."""
+    _LAZY = ("observations", "actions", "rewards", "returns", "advantages", "agent_infos", "env_infos", "paths",
+             "valids")
 
     def __init__(self, batch, paths):
         dict.__init__(self, lane_batch=batch)
         self.lane_batch = batch
         self._paths = paths
 
+    def _recurrent(self, key):
+        return recurrent_samples_entry(self._paths.to_paths(), key)
+
     def __missing__(self, key):
         if key not in self._LAZY:
             raise KeyError(key)
         b = self.lane_batch
+        if getattr(b, "recurrent", False):
+            v = self[key] = self._recurrent(key)
+            return v
+        if key == "valids":
+            raise KeyError(key)
         import torch
         from .. import ops
 
@@ -130,6 +167,8 @@ class SamplesData(dict):
         return v
 
     def __contains__(self, key):
+        if key == "valids":
+            return bool(getattr(self.lane_batch, "recurrent", False))
         return dict.__contains__(self, key) or key in self._LAZY
 
 
@@ -171,6 +210,8 @@ class LaneSampler(Sampler):
         pol = algo.policy
         self.batch = ops.LaneBatch(pol.obs_dim, pol.action_dim, n_local, T, dev)
         self.batch.categorical = ops.is_categorical(pol.dims)
+        self.batch.recurrent = ops.is_gru(pol.dims)
+        self.batch.prev_action_info = self.batch.recurrent and bool(pol.state_include_action)
         if self.batch.categorical != (ops.env_num_actions(self.env_kind) > 0):
             raise TypeError("the policy's action distribution does not match the env's action space")
         self.batch.B_global = n_total * T
@@ -189,8 +230,12 @@ class LaneSampler(Sampler):
     def obtain_samples(self, itr):
         from .. import ops
         algo, b, pol = self.algo, self.batch, self.algo.policy
-        ops.rollout(self.env_kind, pol.theta32, pol.h1, pol.h2, pol.min_std, b, int(algo.max_path_length), None, None,
-                    int(self.seed) & 0xFFFFFFFF, int(itr) & 0xFFFFFFFF, self.lane0)
+        if b.recurrent:
+            ops.gru_rollout(pol.dims, pol.theta32, b, int(algo.max_path_length), self.env_kind, None, None,
+                            int(self.seed) & 0xFFFFFFFF, int(itr) & 0xFFFFFFFF, self.lane0)
+        else:
+            ops.rollout(self.env_kind, pol.theta32, pol.h1, pol.h2, pol.min_std, b, int(algo.max_path_length), None, None,
+                        int(self.seed) & 0xFFFFFFFF, int(itr) & 0xFFFFFFFF, self.lane0)
         b.version += 1
         b.processed = False
         b.masked = False
