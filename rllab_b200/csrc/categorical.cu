@@ -185,22 +185,11 @@ __device__ __forceinline__ void cat_logit_hvp(const T (&p)[NA], const T (&tz)[NA
 }
 
 // ------------------------------------------------------------------------------------------------ rollout / get_actions
-struct CatRolloutArgs {
-  const float* params;
-  int N, T, max_path_length;
-  const float* u;
-  const float* reset_raw;
-  uint32_t seed, iter;
-  long long lane0;
-  float *obs, *act, *prob, *rew;
-  unsigned char* flags;
-  unsigned short* tstep;
-};
-
-// One thread per lane, as rollout_kernel: the policy head draws action = weighted_sample(prob, u) and the env takes the
-// index; act holds the one-hot action (the reference's flattened action, sampler/utils.py:23), prob the probabilities.
+// One thread per lane (lane_rollout, envs.cuh): the policy head draws action = weighted_sample(prob, u) with u from
+// a.eps, and the env takes the index; act holds the one-hot action (the reference's flattened action,
+// sampler/utils.py:23), the mean plane the probabilities.
 template <class Env>
-__global__ void __launch_bounds__(128, 4) cat_rollout_kernel(CatRolloutArgs a) {
+__global__ void __launch_bounds__(128, 4) cat_rollout_kernel(RolloutArgs a) {
   using N_ = CatNet;
   static_assert(Env::O == N_::O && EnvNumActions<Env>::value == N_::A, "env and categorical net disagree");
   __shared__ __align__(16) float sp[(CAT_P + 3) & ~3];
@@ -209,41 +198,24 @@ __global__ void __launch_bounds__(128, 4) cat_rollout_kernel(CatRolloutArgs a) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= a.N) return;
   const long long lane = a.lane0 + n;
-  const size_t N = a.N, TN = (size_t)a.T * a.N;
-  float s[Env::S];
-  draw_reset<Env>(s, a.reset_raw, 0, a.N, n, a.seed, a.iter, lane);
-  int plen = 0;
-  for (int t = 0; t < a.T; ++t) {
-    float o[Env::O], h1[CAT_H], h2[CAT_H], z[CAT_N], p[CAT_N];
-    asm volatile("" ::: "memory");
-    Env::obs(s, o);
-    mlp_forward_thread<N_>(sp, o, h1, h2, z);
-    cat_softmax(z, p);
-    const int k_act = cat_sample(p, cat_draw_u(a.u, t, a.N, n, a.seed, a.iter, lane));
-    const size_t idx = (size_t)t * N + n;
+  float p[CAT_N];
+  int k_act;
+  lane_rollout<Env>(
+      a, n,
+      [&](int t, int, const float (&o)[Env::O]) {
+        float h1[CAT_H], h2[CAT_H], z[CAT_N];
+        mlp_forward_thread<N_>(sp, o, h1, h2, z);
+        cat_softmax(z, p);
+        k_act = cat_sample(p, cat_draw_u(a.eps, t, a.N, n, a.seed, a.iter, lane));
+      },
+      [&](size_t idx, size_t TN, float (&u)[Env::A]) {
 #pragma unroll
-    for (int k = 0; k < Env::O; ++k) a.obs[k * TN + idx] = o[k];
-#pragma unroll
-    for (int k = 0; k < CAT_N; ++k) {
-      a.act[k * TN + idx] = (k == k_act) ? 1.0f : 0.0f;
-      a.prob[k * TN + idx] = p[k];
-    }
-    const float uu[Env::A] = {(float)k_act};
-    float r;
-    bool done;
-    Env::step(s, uu, r, done);
-    a.tstep[idx] = (unsigned short)plen;
-    ++plen;
-    const bool whole = done || (plen >= a.max_path_length);
-    const bool end = whole || (t == a.T - 1);
-    a.rew[idx] = r;
-    a.flags[idx] = (unsigned char)((done ? B200RL_FLAG_DONE : 0) | (end ? B200RL_FLAG_END : 0) |
-                                   ((end && !whole) ? B200RL_FLAG_CUT : 0));
-    if (end) {
-      draw_reset<Env>(s, a.reset_raw, t + 1, a.N, n, a.seed, a.iter, lane);
-      plen = 0;
-    }
-  }
+        for (int k = 0; k < CAT_N; ++k) {
+          a.act[k * TN + idx] = (k == k_act) ? 1.0f : 0.0f;
+          a.mean[k * TN + idx] = p[k];
+        }
+        u[0] = (float)k_act;
+      });
 }
 
 __global__ void __launch_bounds__(128) cat_get_actions_kernel(const float* __restrict__ params,
@@ -523,14 +495,10 @@ static int launch_cat_tile(const UpdArgs& a, int* grid_out, cudaStream_t st) {
   int per_sm = (int)((228 * 1024) / (SM::bytes + 1024));
   if (per_sm < 1) per_sm = 1;
   if (per_sm > cat_tile_minblocks<MODE>()) per_sm = cat_tile_minblocks<MODE>();
-  long long grid = (long long)num_sms() * per_sm;
-  const long long ntiles = host_n_tiles(a, CT_TILE);
-  if (grid > ntiles) grid = ntiles;
-  if (grid > MAX_PARTIAL_BLOCKS) grid = MAX_PARTIAL_BLOCKS;
-  if (grid < 1) grid = 1;
-  cat_tile_kernel<MODE><<<(unsigned)grid, CT_THREADS, SM::bytes, st>>>(a);
+  const int grid = partial_grid(per_sm, host_n_tiles(a, CT_TILE));
+  cat_tile_kernel<MODE><<<grid, CT_THREADS, SM::bytes, st>>>(a);
   B200RL_LAUNCH_CHECK("cat_tile_kernel");
-  *grid_out = (int)grid;
+  *grid_out = grid;
   return 0;
 }
 
@@ -796,21 +764,15 @@ int b200rl_rollout_categorical(int env_kind, const float* params_f32, int h1, in
                                int max_path_length, const float* u, const float* reset_raw, unsigned int seed,
                                unsigned int iter, long long lane0, float* obs, float* act, float* prob, float* rew,
                                unsigned char* flags, unsigned short* tstep, void* stream) {
-  B200RL_REQUIRE(params_f32 && obs && act && prob && rew && flags && tstep, "rollout_categorical: null buffer");
-  B200RL_REQUIRE(N > 0 && T > 0 && max_path_length > 0, "rollout_categorical: N, T, max_path_length must be positive");
-  B200RL_REQUIRE(max_path_length <= 65535, "rollout_categorical: max_path_length must fit uint16 tstep");
+  const RolloutArgs a{params_f32, 0.f, N, T, max_path_length, u, reset_raw, seed, iter, lane0,
+                      obs, act, prob, rew, flags, tstep, nullptr};
+  if (int rc = check_rollout_args("rollout_categorical", a, false)) return rc;
   if (env_kind != B200RL_ENV_GYM_CARTPOLE) {
     set_error("rollout_categorical: env kind %d has no discrete action space compiled in (only %d, CartPole-v0)",
               env_kind, B200RL_ENV_GYM_CARTPOLE);
     return B200RL_EUNSUPPORTED;
   }
   B200RL_REQUIRE_CAT_SHAPE(GymCartPoleEnvD::O, h1, h2, EnvNumActions<GymCartPoleEnvD>::value, "rollout_categorical");
-  CatRolloutArgs a;
-  a.params = params_f32;
-  a.N = N; a.T = T; a.max_path_length = max_path_length;
-  a.u = u; a.reset_raw = reset_raw;
-  a.seed = seed; a.iter = iter; a.lane0 = lane0;
-  a.obs = obs; a.act = act; a.prob = prob; a.rew = rew; a.flags = flags; a.tstep = tstep;
   cat_rollout_kernel<GymCartPoleEnvD><<<(N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(a);
   B200RL_LAUNCH_CHECK("cat_rollout_kernel");
   return 0;
@@ -821,23 +783,15 @@ int b200rl_categorical_loss_kl(int loss_kind, const float* params_f32, int obs_d
                                const float* old_prob, const unsigned char* flags, double scale, const double* count,
                                double* out, double* ws, void* stream) {
   B200RL_REQUIRE(params_f32 && obs && act && adv && old_prob && out && ws && B > 0, "categorical_loss_kl: bad arguments");
-  B200RL_REQUIRE(loss_kind == B200RL_LOSS_TRPO || loss_kind == B200RL_LOSS_VPG, "categorical_loss_kl: bad loss kind");
+  if (int rc = check_loss_kind("categorical_loss_kl", loss_kind)) return rc;
   B200RL_REQUIRE_CAT_SHAPE(obs_dim, h1, h2, n_actions, "categorical_loss_kl");
   cudaStream_t st = (cudaStream_t)stream;
   UpdArgs a{};
   cat_fill_args(a, params_f32, B, obs, act, adv, old_prob, loss_kind, flags, ws);
-  long long g = (long long)num_sms() * 4;
-  const long long need = (B + 127) / 128;
-  if (g > need) g = need;
-  if (g > MAX_PARTIAL_BLOCKS) g = MAX_PARTIAL_BLOCKS;
-  const int grid = (int)g;
+  const int grid = partial_grid(4, (B + 127) / 128);
   cat_loss_kernel<<<grid, 128, 0, st>>>(a);
   B200RL_LAUNCH_CHECK("cat_loss_kernel");
-  FinArgs f{};
-  f.partial = nullptr; f.nblocks = grid; f.K = 0; f.vec_out = nullptr;
-  f.tri_partial = ws; f.NT = 3; f.tri_out = out; f.scale = scale; f.count = count; f.post = FIN_NONE;
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  return launch_finalize_update(fin_loss(ws, grid, out, scale, count), st);
 }
 
 int b200rl_categorical_grad(int loss_kind, double penalty, const float* params_f32, int obs_dim, int h1, int h2,
@@ -845,7 +799,7 @@ int b200rl_categorical_grad(int loss_kind, double penalty, const float* params_f
                             const float* old_prob, const unsigned char* flags, double scale, const double* count,
                             double* g_out, double* loss_out, float* h_cache_out, double* ws, void* stream) {
   B200RL_REQUIRE(params_f32 && obs && act && adv && old_prob && g_out && ws && B > 0, "categorical_grad: bad arguments");
-  B200RL_REQUIRE(loss_kind == B200RL_LOSS_TRPO || loss_kind == B200RL_LOSS_VPG, "categorical_grad: bad loss kind");
+  if (int rc = check_loss_kind("categorical_grad", loss_kind)) return rc;
   B200RL_REQUIRE(penalty >= 0.0 && penalty <= 3.0e38, "categorical_grad: penalty must be finite and >= 0");
   B200RL_REQUIRE_CAT_SHAPE(obs_dim, h1, h2, n_actions, "categorical_grad");
   cudaStream_t st = (cudaStream_t)stream;
@@ -856,12 +810,9 @@ int b200rl_categorical_grad(int loss_kind, double penalty, const float* params_f
   int grid = 0;
   int rc = penalty == 0.0 ? launch_cat_tile<MODE_GRAD>(a, &grid, st) : launch_cat_tile<MODE_GRAD_KL>(a, &grid, st);
   if (rc) return rc;
-  FinArgs f{};
-  f.partial = ws; f.nblocks = grid; f.K = CAT_P; f.vec_out = g_out;
-  f.tri_partial = ws + (size_t)grid * CAT_P; f.NT = 3; f.tri_out = loss_out;
-  f.scale = scale; f.count = count; f.post = FIN_NONE; f.ols = CAT_P; f.A = 0;
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  // no log_std block (A = 0): the gradient's min_std mask touches no entry
+  return launch_finalize_update(fin_grad(ws, grid, CAT_P, g_out, loss_out, scale, count, {CAT_P, 0, nullptr, nullptr, 0.0}),
+                                st);
 }
 
 int b200rl_categorical_fvp(const float* params_f32, int obs_dim, int h1, int h2, int n_actions, long long B,
@@ -878,12 +829,9 @@ int b200rl_categorical_fvp(const float* params_f32, int obs_dim, int h1, int h2,
   int grid = 0;
   int rc = launch_cat_tile<MODE_FVP>(a, &grid, st);
   if (rc) return rc;
-  FinArgs f{};
-  f.partial = ws; f.nblocks = grid; f.K = CAT_P; f.vec_out = Hx_out; f.tri_out = nullptr;
-  f.scale = scale; f.count = count; f.post = FIN_FVP; f.ols = CAT_P; f.A = 0;   // no log_std block
-  f.params32 = params_f32; f.x = x; f.reg = reg_coeff; f.diag_scale = diag_scale;
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  return launch_finalize_update(fin_fvp(ws, grid, CAT_P, Hx_out, scale, count, {CAT_P, 0, params_f32, nullptr, 0.0}, x,
+                                        reg_coeff, diag_scale),   // no log_std block
+                                st);
 }
 
 int b200rl_categorical_update_f64(int mode, int loss_kind, const double* params_f64, int obs_dim, int h1, int h2,
@@ -892,12 +840,8 @@ int b200rl_categorical_update_f64(int mode, int loss_kind, const double* params_
                                   const double* count, double reg_coeff, double diag_scale, double* vec_out,
                                   double* loss_out, double* ws, void* stream) {
   B200RL_REQUIRE(params_f64 && obs && ws && B > 0, "categorical_update_f64: bad arguments");
-  B200RL_REQUIRE(mode == MODE_LOSS || mode == MODE_GRAD || mode == MODE_FVP, "categorical_update_f64: bad mode");
-  B200RL_REQUIRE(mode == MODE_FVP ? (x && vec_out) : (act && adv && old_prob), "categorical_update_f64: null buffer");
-  B200RL_REQUIRE(mode != MODE_GRAD || vec_out, "categorical_update_f64: gradient output missing");
-  B200RL_REQUIRE(mode != MODE_LOSS || loss_out, "categorical_update_f64: loss output missing");
-  B200RL_REQUIRE(loss_kind == B200RL_LOSS_TRPO || loss_kind == B200RL_LOSS_VPG ||
-                 (loss_kind == B200RL_LOSS_KL && mode == MODE_GRAD), "categorical_update_f64: bad loss kind");
+  if (int rc = check_f64_args("categorical_update_f64", mode, loss_kind, act && adv && old_prob, x, vec_out, loss_out))
+    return rc;
   B200RL_REQUIRE_CAT_SHAPE(obs_dim, h1, h2, n_actions, "categorical_update_f64");
   cudaStream_t st = (cudaStream_t)stream;
   CatArgs64 a{};
@@ -908,16 +852,9 @@ int b200rl_categorical_update_f64(int mode, int loss_kind, const double* params_
          : (mode == MODE_GRAD) ? launch_cat_f64<MODE_GRAD>(a, &grid, st)
                                : launch_cat_f64<MODE_FVP>(a, &grid, st);
   if (rc) return rc;
-  FinArgs f{};
-  f.nblocks = grid; f.scale = scale; f.count = count; f.ols = CAT_P; f.A = 0; f.post = FIN_NONE;
-  if (mode != MODE_LOSS) { f.partial = ws; f.K = CAT_P; f.vec_out = vec_out; }
-  if (mode == MODE_FVP) { f.post = FIN_FVP; f.params64 = params_f64; f.x = x; f.reg = reg_coeff; f.diag_scale = diag_scale; }
-  if (mode != MODE_FVP && loss_out != nullptr) {
-    f.tri_partial = (mode == MODE_LOSS) ? ws : ws + (size_t)grid * CAT_P;
-    f.NT = 3; f.tri_out = loss_out;
-  }
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  return launch_finalize_update(fin_f64(mode, ws, grid, CAT_P, vec_out, loss_out, scale, count,
+                                        {CAT_P, 0, nullptr, params_f64, 0.0}, x, reg_coeff, diag_scale),
+                                st);
 }
 
 int b200rl_categorical_entropy(int n_actions, long long B, const float* prob, const unsigned char* flags, double* out,
@@ -928,12 +865,9 @@ int b200rl_categorical_entropy(int n_actions, long long B, const float* prob, co
     return B200RL_EUNSUPPORTED;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  long long g = (long long)num_sms() * 4;
-  const long long need = (B + 255) / 256;
-  if (g > need) g = need;
-  if (g > MAX_PARTIAL_BLOCKS) g = MAX_PARTIAL_BLOCKS;
-  cat_entropy_kernel<<<(unsigned)g, 256, 0, st>>>(B, prob, flags, ws);
+  const int grid = partial_grid(4, (B + 255) / 256);
+  cat_entropy_kernel<<<grid, 256, 0, st>>>(B, prob, flags, ws);
   B200RL_LAUNCH_CHECK("cat_entropy_kernel");
-  return launch_finalize_sum(ws, (int)g, 2, out, 1.0, st);
+  return launch_finalize_sum(ws, grid, 2, out, 1.0, st);
 }
 }

@@ -30,6 +30,13 @@ int num_sms() {
   return sms;
 }
 
+int partial_grid(int blocks_per_sm, long long work) {
+  long long g = (long long)num_sms() * blocks_per_sm;
+  if (g > work) g = work;
+  if (g > MAX_PARTIAL_BLOCKS) g = MAX_PARTIAL_BLOCKS;
+  return (int)(g < 1 ? 1 : g);
+}
+
 // out[k] = op over blocks of partial[b][k].  32 outputs x FIN_SLICES block-slices per CTA: each slice walks every
 // FIN_SLICES-th block (coalesced 256 B rows, 4 loads in flight), the slices are combined through shared memory in fixed
 // order, so the result is deterministic and the dependent-add chain is nblocks/FIN_SLICES long instead of nblocks.
@@ -176,10 +183,67 @@ __global__ void __launch_bounds__(FIN_THREADS) finalize_update_kernel(FinArgs f)
   }
 }
 
-int launch_finalize_update(const FinArgs& f, cudaStream_t s) {
+int launch_finalize_update(FinArgs f, cudaStream_t s) {
+  if (peer_fused()) f.peer = peer_next();
   const int nvb = (f.K + 31) / 32;
   finalize_update_kernel<<<nvb + (f.tri_out != nullptr ? 1 : 0), FIN_THREADS, 0, s>>>(f);
   B200RL_LAUNCH_CHECK("finalize_update_kernel");
+  return 0;
+}
+
+FinArgs fin_loss(const double* ws, int grid, double* tri_out, double scale, const double* count) {
+  FinArgs f{};
+  f.nblocks = grid;
+  f.tri_partial = ws; f.NT = 3; f.tri_out = tri_out;
+  f.scale = scale; f.count = count; f.post = FIN_NONE;
+  return f;
+}
+
+static void set_log_std(FinArgs& f, const LogStdBlock& ls) {
+  f.ols = ls.ols; f.A = ls.A;
+  f.params32 = ls.params32; f.params64 = ls.params64; f.log_min_std = ls.log_min_std;
+}
+
+FinArgs fin_grad(const double* ws, int grid, int P, double* vec_out, double* tri_out, double scale, const double* count,
+                 const LogStdBlock& ls) {
+  FinArgs f{};
+  f.partial = ws; f.nblocks = grid; f.K = P; f.vec_out = vec_out;
+  f.tri_partial = ws + (size_t)grid * P; f.NT = 3; f.tri_out = tri_out;
+  f.scale = scale; f.count = count; f.post = FIN_GRAD;
+  set_log_std(f, ls);
+  return f;
+}
+
+FinArgs fin_fvp(const double* ws, int grid, int P, double* vec_out, double scale, const double* count,
+                const LogStdBlock& ls, const double* x, double reg, double diag_scale) {
+  FinArgs f{};
+  f.partial = ws; f.nblocks = grid; f.K = P; f.vec_out = vec_out;
+  f.scale = scale; f.count = count; f.post = FIN_FVP;
+  set_log_std(f, ls);
+  f.x = x; f.reg = reg; f.diag_scale = diag_scale;
+  return f;
+}
+
+FinArgs fin_f64(int mode, const double* ws, int grid, int P, double* vec_out, double* tri_out, double scale,
+                const double* count, const LogStdBlock& ls, const double* x, double reg, double diag_scale) {
+  if (mode == MODE_LOSS) return fin_loss(ws, grid, tri_out, scale, count);
+  if (mode == MODE_GRAD) return fin_grad(ws, grid, P, vec_out, tri_out, scale, count, ls);
+  return fin_fvp(ws, grid, P, vec_out, scale, count, ls, x, reg, diag_scale);
+}
+
+int check_loss_kind(const char* entry, int loss_kind) {
+  B200RL_REQUIRE(loss_kind == B200RL_LOSS_TRPO || loss_kind == B200RL_LOSS_VPG, "%s: bad loss kind", entry);
+  return 0;
+}
+
+int check_f64_args(const char* entry, int mode, int loss_kind, bool inputs_ok, const double* x, const double* vec_out,
+                   const double* loss_out) {
+  B200RL_REQUIRE(mode == MODE_LOSS || mode == MODE_GRAD || mode == MODE_FVP, "%s: bad mode", entry);
+  B200RL_REQUIRE(mode == MODE_FVP ? (x && vec_out) : inputs_ok, "%s: null buffer", entry);
+  B200RL_REQUIRE(mode != MODE_GRAD || vec_out, "%s: gradient output missing", entry);
+  B200RL_REQUIRE(mode != MODE_LOSS || loss_out, "%s: loss output missing", entry);
+  B200RL_REQUIRE(loss_kind == B200RL_LOSS_TRPO || loss_kind == B200RL_LOSS_VPG ||
+                 (loss_kind == B200RL_LOSS_KL && mode == MODE_GRAD), "%s: bad loss kind", entry);
   return 0;
 }
 

@@ -56,6 +56,9 @@ int num_sms();
 // writes [block][K] float64 partials; K <= MAX_PARTIAL_K.  (8 blocks per SM on GPUs of up to 148 SMs.)
 constexpr int MAX_PARTIAL_BLOCKS = 148 * 8;
 constexpr int MAX_PARTIAL_K = 8192;
+// Grid of a pass that writes per-block partials: blocks_per_sm CTAs per SM, no more than the `work` blocks that have
+// samples, no more than MAX_PARTIAL_BLOCKS, at least one.
+int partial_grid(int blocks_per_sm, long long work);
 
 // ---------------------------------------------------------------- Philox4x32-10 (Salmon et al. 2011)
 struct Philox {
@@ -180,6 +183,9 @@ int launch_finalize_max(const double* partial, int nblocks, int K, double* out, 
 //   peer.world > 1   : the vector and the tuple are additionally reduced over the ranks of the bound peer-memory
 //                      communicator in the same launch (peer.cuh): sums (and the tuple's max) of every rank's result
 constexpr int FIN_NONE = 0, FIN_GRAD = 1, FIN_FVP = 2;
+// Policy-update pass modes.  MODE_GRAD_KL: MODE_GRAD plus penalty * (gradient of the per-sample KL(old || new)), the
+// objective of the penalised L-BFGS policy update (tensor-core kernels only: update_umma.cu, update_umma32.cu)
+constexpr int MODE_LOSS = 0, MODE_GRAD = 1, MODE_FVP = 2, MODE_GRAD_KL = 3;
 constexpr int PEER_MAX_RANKS = B200RL_PEER_MAX_RANKS;
 struct PeerArgs {
   unsigned char* win[PEER_MAX_RANKS];   // exchange-window base pointers, indexed by rank (entry `rank` = own window)
@@ -198,6 +204,36 @@ struct FinArgs {
   const double* x; double reg, diag_scale;
   PeerArgs peer;
 };
-int launch_finalize_update(const FinArgs& f, cudaStream_t s);
+// Launches finalize_update_kernel; with peer fusion enabled it also takes the next collective's sequence number, so a
+// call rejected before this point consumes none.
+int launch_finalize_update(FinArgs f, cudaStream_t s);
+
+// The four shapes a policy-update pass finishes with.  A pass's workspace `ws` holds its per-block vector partials
+// [grid][P], then its per-block (loss, sum KL, max KL) triples [grid][3] behind them; a loss-only pass writes the triples
+// alone.  A triple output of NULL skips the triple.
+//   LogStdBlock: entries [ols, ols + A) of the parameters (params32 or params64) are log_std with the min_std clamp
+//   log_min_std; the gradient's clamp mask and the Fisher product's log_std diagonal apply there (A = 0: none).
+struct LogStdBlock {
+  int ols, A;
+  const float* params32;
+  const double* params64;
+  double log_min_std;
+};
+FinArgs fin_loss(const double* ws, int grid, double* tri_out, double scale, const double* count);
+FinArgs fin_grad(const double* ws, int grid, int P, double* vec_out, double* tri_out, double scale, const double* count,
+                 const LogStdBlock& ls);
+FinArgs fin_fvp(const double* ws, int grid, int P, double* vec_out, double scale, const double* count,
+                const LogStdBlock& ls, const double* x, double reg, double diag_scale);
+// float64 parity pass: MODE_LOSS as fin_loss, MODE_GRAD as fin_grad (tri_out may be NULL), MODE_FVP as fin_fvp.
+FinArgs fin_f64(int mode, const double* ws, int grid, int P, double* vec_out, double* tri_out, double scale,
+                const double* count, const LogStdBlock& ls, const double* x, double reg, double diag_scale);
+
+// Checks of the policy-update entry points; `entry` prefixes the error text.
+// loss kind of a surrogate pass: B200RL_LOSS_TRPO or B200RL_LOSS_VPG
+int check_loss_kind(const char* entry, int loss_kind);
+// float64 parity pass: the mode, its buffers (inputs_ok: the loss and gradient modes' sample inputs are non-NULL) and
+// the loss kind (B200RL_LOSS_KL, the gradient of mean KL, in MODE_GRAD only)
+int check_f64_args(const char* entry, int mode, int loss_kind, bool inputs_ok, const double* x, const double* vec_out,
+                   const double* loss_out);
 
 }  // namespace b200rl

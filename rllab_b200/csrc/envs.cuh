@@ -307,6 +307,77 @@ __device__ __forceinline__ void draw_eps(float (&e)[A], const float* __restrict_
   }
 }
 
+// Arguments of the fused lane rollouts (rollout_kernel, cat_rollout_kernel, gru_rollout_kernel).  eps: the action noise
+// [T][A][N] (the categorical rollout's uniforms [T][N]) or NULL for Philox; mean: the mean plane (the categorical
+// rollout's probabilities); log_min_std, log_std_out: the Gaussian policies' log_std only.
+struct RolloutArgs {
+  const float* params;
+  float log_min_std;
+  int N, T, max_path_length;
+  const float* eps;
+  const float* reset_raw;
+  uint32_t seed, iter;
+  long long lane0;
+  float *obs, *act, *mean, *rew;
+  unsigned char* flags;
+  unsigned short* tstep;
+  float* log_std_out;
+};
+
+// The checks the fused rollouts' entry points make first; `entry` prefixes the error text.  with_log_std: the policy
+// has a log_std to report (log_std_out required).
+inline int check_rollout_args(const char* entry, const RolloutArgs& a, bool with_log_std) {
+  B200RL_REQUIRE(a.params && a.obs && a.act && a.mean && a.rew && a.flags && a.tstep &&
+                 (a.log_std_out || !with_log_std), "%s: null buffer", entry);
+  B200RL_REQUIRE(a.N > 0 && a.T > 0 && a.max_path_length > 0, "%s: N, T, max_path_length must be positive", entry);
+  B200RL_REQUIRE(a.max_path_length <= 65535, "%s: max_path_length must fit uint16 tstep", entry);
+  return 0;
+}
+
+// The lane loop of the fused rollouts: lane n runs all T steps in one thread with the env state in registers.  The loop
+// owns the sample bookkeeping that process_samples, the whole-path masking, REPS and the GRU passes read: obs and rew
+// planes, tstep (the step's index in its path, so a path starts where tstep == 0), the DONE / END / CUT flags, and the
+// resets (row 0 for the first path, row t + 1 after a path ends at step t).  The policy's head runs in two calls per step:
+//   act(t, plen, o)      computes the action from the observation o (plen == 0: the first step of a path);
+//   record(idx, TN, u)   writes the policy's act and mean planes at [k * TN + idx] and returns the env input in u.
+// The obs plane is stored between the two, after the noise loads and before the act / mean stores: the compiler may not
+// reorder these possibly aliasing accesses, and any other order changes the hot rollout's generated code.
+template <class Env, class Act, class Record>
+__device__ __forceinline__ void lane_rollout(const RolloutArgs& a, int n, Act&& act, Record&& record) {
+  const long long lane = a.lane0 + n;
+  const size_t N = a.N, TN = (size_t)a.T * a.N;
+  float s[Env::S];
+  draw_reset<Env>(s, a.reset_raw, 0, a.N, n, a.seed, a.iter, lane);
+  int plen = 0;
+  for (int t = 0; t < a.T; ++t) {
+    float o[Env::O], u[Env::A];
+    // compiler barrier: without it the loop-invariant LDS of all P weights is hoisted out of the t loop and spilled
+    asm volatile("" ::: "memory");
+    Env::obs(s, o);
+    act(t, plen, o);
+    const size_t idx = (size_t)t * N + n;
+#pragma unroll
+    for (int k = 0; k < Env::O; ++k) a.obs[k * TN + idx] = o[k];
+    record(idx, TN, u);
+    float r;
+    bool done;
+    Env::step(s, u, r, done);
+    a.tstep[idx] = (unsigned short)plen;
+    ++plen;
+    const bool whole = done || (plen >= a.max_path_length);
+    const bool end = whole || (t == a.T - 1);
+    a.rew[idx] = r;
+    // FLAG_CUT: the path is cut by the end of the lane buffer, not by the env or max_path_length (process_samples drops
+    // such paths when the caller asks for whole paths only, batch_polopt.py:30-34)
+    a.flags[idx] = (unsigned char)((done ? B200RL_FLAG_DONE : 0) | (end ? B200RL_FLAG_END : 0) |
+                                   ((end && !whole) ? B200RL_FLAG_CUT : 0));
+    if (end) {
+      draw_reset<Env>(s, a.reset_raw, t + 1, a.N, n, a.seed, a.iter, lane);
+      plen = 0;
+    }
+  }
+}
+
 // Dispatch an env kind to its struct: F is a generic lambda / functor called as f(Env{}).
 #define B200RL_DISPATCH_ENV(kind, ...)                                                        \
   switch (kind) {                                                                             \

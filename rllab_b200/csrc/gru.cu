@@ -112,22 +112,9 @@ __device__ __forceinline__ void gru_input(const float* __restrict__ obs, const f
 }
 
 // ------------------------------------------------------------------------------------------------ rollout / get_actions
-struct GruRolloutArgs {
-  const float* params;
-  int N, T, max_path_length;
-  const float* eps;
-  const float* reset_raw;
-  uint32_t seed, iter;
-  long long lane0;
-  float *obs, *act, *mean, *rew;
-  unsigned char* flags;
-  unsigned short* tstep;
-  float* log_std_out;
-};
-
-// One thread per lane for all T steps (rollout_kernel's layout): env state, h and prev_action in registers.
+// One thread per lane for all T steps (lane_rollout, envs.cuh): env state, h and prev_action in registers.
 template <class Env, class N_>
-__global__ void __launch_bounds__(128) gru_rollout_kernel(GruRolloutArgs a) {
+__global__ void __launch_bounds__(128) gru_rollout_kernel(RolloutArgs a) {
   static_assert(Env::O == N_::O && Env::A == N_::A, "env and GRU net disagree");
   constexpr int H = N_::H, A = N_::A;
   __shared__ __align__(16) float sp[N_::P4];
@@ -142,54 +129,36 @@ __global__ void __launch_bounds__(128) gru_rollout_kernel(GruRolloutArgs a) {
   }
   if (n >= a.N) return;
   const long long lane = a.lane0 + n;
-  const size_t N = a.N, TN = (size_t)a.T * a.N;
-  float s[Env::S], h[H], pa[A];
-  draw_reset<Env>(s, a.reset_raw, 0, a.N, n, a.seed, a.iter, lane);
-  int plen = 0;
-  for (int t = 0; t < a.T; ++t) {
-    asm volatile("" ::: "memory");
-    if (plen == 0) {   // path start: h_0 = 0, prev_action = 0
+  float h[H], pa[A], hn[H], mu[A], e[A];
+  lane_rollout<Env>(
+      a, n,
+      [&](int t, int plen, const float (&o)[Env::O]) {
+        if (plen == 0) {   // path start: h_0 = 0, prev_action = 0
 #pragma unroll
-      for (int j = 0; j < H; ++j) h[j] = 0.f;
+          for (int j = 0; j < H; ++j) h[j] = 0.f;
 #pragma unroll
-      for (int k = 0; k < A; ++k) pa[k] = 0.f;
-    }
-    float o[Env::O], x[N_::I], hn[H], mu[A], e[A], u[A];
-    Env::obs(s, o);
+          for (int k = 0; k < A; ++k) pa[k] = 0.f;
+        }
+        float x[N_::I];
 #pragma unroll
-    for (int k = 0; k < Env::O; ++k) x[k] = o[k];
+        for (int k = 0; k < Env::O; ++k) x[k] = o[k];
 #pragma unroll
-    for (int k = 0; k < N_::I - N_::O; ++k) x[N_::O + k] = pa[k];
-    gru_cell<N_>(sp, x, h, hn);
-    gru_mean<N_>(sp, hn, mu);
-    draw_eps<A>(e, a.eps, t, a.N, n, a.seed, a.iter, lane);
-    const size_t idx = (size_t)t * N + n;
+        for (int k = 0; k < N_::I - N_::O; ++k) x[N_::O + k] = pa[k];
+        gru_cell<N_>(sp, x, h, hn);
+        gru_mean<N_>(sp, hn, mu);
+        draw_eps<A>(e, a.eps, t, a.N, n, a.seed, a.iter, lane);
+      },
+      [&](size_t idx, size_t TN, float (&u)[A]) {
 #pragma unroll
-    for (int k = 0; k < Env::O; ++k) a.obs[k * TN + idx] = o[k];
+        for (int k = 0; k < A; ++k) {
+          pa[k] = fmaf(std_[k], e[k], mu[k]);   // rnd * exp(log_std) + mean (gaussian_gru_policy.py:get_action)
+          u[k] = scale_action(pa[k], Env::lb(k), Env::ub(k));
+          a.act[k * TN + idx] = pa[k];
+          a.mean[k * TN + idx] = mu[k];
+        }
 #pragma unroll
-    for (int k = 0; k < A; ++k) {
-      pa[k] = fmaf(std_[k], e[k], mu[k]);   // rnd * exp(log_std) + mean (gaussian_gru_policy.py:get_action)
-      u[k] = scale_action(pa[k], Env::lb(k), Env::ub(k));
-      a.act[k * TN + idx] = pa[k];
-      a.mean[k * TN + idx] = mu[k];
-    }
-#pragma unroll
-    for (int j = 0; j < H; ++j) h[j] = hn[j];
-    float r;
-    bool done;
-    Env::step(s, u, r, done);
-    a.tstep[idx] = (unsigned short)plen;
-    ++plen;
-    const bool whole = done || (plen >= a.max_path_length);
-    const bool end = whole || (t == a.T - 1);
-    a.rew[idx] = r;
-    a.flags[idx] = (unsigned char)((done ? B200RL_FLAG_DONE : 0) | (end ? B200RL_FLAG_END : 0) |
-                                   ((end && !whole) ? B200RL_FLAG_CUT : 0));
-    if (end) {
-      draw_reset<Env>(s, a.reset_raw, t + 1, a.N, n, a.seed, a.iter, lane);
-      plen = 0;
-    }
-  }
+        for (int j = 0; j < H; ++j) h[j] = hn[j];
+      });
 }
 
 template <class N_>
@@ -646,13 +615,10 @@ template <class N_, int MODE>
 static int launch_gru_bptt(const GruArgs& a, int* grid_out, cudaStream_t st) {
   using S = GruStage<N_>;
   B200RL_SET_MAX_SMEM((gru_bptt_kernel<N_, MODE>), S::bytes);
-  long long grid = num_sms();
-  const long long ntiles = (a.N + GT - 1) / GT;
-  if (grid > ntiles) grid = ntiles;
-  if (grid > MAX_PARTIAL_BLOCKS) grid = MAX_PARTIAL_BLOCKS;
-  gru_bptt_kernel<N_, MODE><<<(unsigned)grid, GT, S::bytes, st>>>(a);
+  const int grid = partial_grid(1, (a.N + GT - 1) / GT);
+  gru_bptt_kernel<N_, MODE><<<grid, GT, S::bytes, st>>>(a);
   B200RL_LAUNCH_CHECK("gru_bptt_kernel");
-  *grid_out = (int)grid;
+  *grid_out = grid;
   return 0;
 }
 
@@ -940,21 +906,15 @@ int b200rl_rollout_gru(int env_kind, const float* params_f32, int hidden, int in
                        int max_path_length, const float* eps, const float* reset_raw, unsigned int seed,
                        unsigned int iter, long long lane0, float* obs, float* act, float* mean, float* rew,
                        unsigned char* flags, unsigned short* tstep, float* log_std_out, void* stream) {
-  B200RL_REQUIRE(params_f32 && obs && act && mean && rew && flags && tstep && log_std_out, "rollout_gru: null buffer");
-  B200RL_REQUIRE(N > 0 && T > 0 && max_path_length > 0, "rollout_gru: N, T, max_path_length must be positive");
-  B200RL_REQUIRE(max_path_length <= 65535, "rollout_gru: max_path_length must fit uint16 tstep");
+  const RolloutArgs a{params_f32, 0.f, N, T, max_path_length, eps, reset_raw, seed, iter, lane0,
+                      obs, act, mean, rew, flags, tstep, log_std_out};
+  if (int rc = check_rollout_args("rollout_gru", a, true)) return rc;
   if (env_kind != B200RL_ENV_CARTPOLE) {
     set_error("rollout_gru: env kind %d is not compiled in for the GRU policy (only %d, CartpoleEnv)", env_kind,
               B200RL_ENV_CARTPOLE);
     return B200RL_EUNSUPPORTED;
   }
   B200RL_REQUIRE_GRU_SHAPE(CartPoleEnvD::O, hidden, CartPoleEnvD::A, "rollout_gru");
-  GruRolloutArgs a;
-  a.params = params_f32;
-  a.N = N; a.T = T; a.max_path_length = max_path_length;
-  a.eps = eps; a.reset_raw = reset_raw;
-  a.seed = seed; a.iter = iter; a.lane0 = lane0;
-  a.obs = obs; a.act = act; a.mean = mean; a.rew = rew; a.flags = flags; a.tstep = tstep; a.log_std_out = log_std_out;
   B200RL_DISPATCH_GRU(include_action, {
     gru_rollout_kernel<CartPoleEnvD, NetG><<<(N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(a);
   });
@@ -969,24 +929,16 @@ int b200rl_gru_loss_kl(int loss_kind, const float* params_f32, int obs_dim, int 
                        double* ws, void* stream) {
   B200RL_REQUIRE(params_f32 && obs && act && tstep && adv && old_mean && old_log_std && out && ws && N > 0 && T > 0,
                  "gru_loss_kl: bad arguments");
-  B200RL_REQUIRE(loss_kind == B200RL_LOSS_TRPO || loss_kind == B200RL_LOSS_VPG, "gru_loss_kl: bad loss kind");
+  if (int rc = check_loss_kind("gru_loss_kl", loss_kind)) return rc;
   B200RL_REQUIRE_GRU_SHAPE(obs_dim, hidden, act_dim, "gru_loss_kl");
   cudaStream_t st = (cudaStream_t)stream;
   GruArgs a{};
   gru_fill(a, params_f32, N, T, obs, act, tstep, adv, old_mean, old_log_std, loss_kind, flags, ws);
   a.hbuf = h_cache_out;
-  long long g = (long long)num_sms() * 4;
-  const long long need = (N + 127) / 128;
-  if (g > need) g = need;
-  if (g > MAX_PARTIAL_BLOCKS) g = MAX_PARTIAL_BLOCKS;
-  const int grid = (int)g;
+  const int grid = partial_grid(4, (N + 127) / 128);
   B200RL_DISPATCH_GRU(include_action, { gru_loss_kernel<NetG><<<grid, 128, 0, st>>>(a); });
   B200RL_LAUNCH_CHECK("gru_loss_kernel");
-  FinArgs f{};
-  f.partial = nullptr; f.nblocks = grid; f.K = 0; f.vec_out = nullptr;
-  f.tri_partial = ws; f.NT = 3; f.tri_out = out; f.scale = scale; f.count = count; f.post = FIN_NONE;
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  return launch_finalize_update(fin_loss(ws, grid, out, scale, count), st);
 }
 
 int b200rl_gru_grad(int loss_kind, double penalty, const float* params_f32, int obs_dim, int hidden, int act_dim,
@@ -996,7 +948,7 @@ int b200rl_gru_grad(int loss_kind, double penalty, const float* params_f32, int 
                     void* stream) {
   B200RL_REQUIRE(params_f32 && obs && act && tstep && adv && old_mean && old_log_std && g_out && h_cache && ws &&
                  N > 0 && T > 0, "gru_grad: bad arguments");
-  B200RL_REQUIRE(loss_kind == B200RL_LOSS_TRPO || loss_kind == B200RL_LOSS_VPG, "gru_grad: bad loss kind");
+  if (int rc = check_loss_kind("gru_grad", loss_kind)) return rc;
   B200RL_REQUIRE(penalty >= 0.0 && penalty <= 3.0e38, "gru_grad: penalty must be finite and >= 0");
   B200RL_REQUIRE_GRU_SHAPE(obs_dim, hidden, act_dim, "gru_grad");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1010,13 +962,8 @@ int b200rl_gru_grad(int loss_kind, double penalty, const float* params_f32, int 
     int rc = launch_gru_bptt<NetG, MODE_GRAD>(a, &grid, st);
     if (rc) return rc;
   });
-  FinArgs f{};
-  f.partial = ws; f.nblocks = grid; f.K = P; f.vec_out = g_out;
-  f.tri_partial = ws + (size_t)grid * P; f.NT = 3; f.tri_out = loss_out;
-  f.scale = scale; f.count = count; f.post = FIN_GRAD; f.ols = ols; f.A = act_dim;
-  f.params32 = params_f32; f.log_min_std = -INFINITY;
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  return launch_finalize_update(
+      fin_grad(ws, grid, P, g_out, loss_out, scale, count, {ols, act_dim, params_f32, nullptr, -INFINITY}), st);
 }
 
 int b200rl_gru_fvp(const float* params_f32, int obs_dim, int hidden, int act_dim, int include_action, int N, int T,
@@ -1042,12 +989,9 @@ int b200rl_gru_fvp(const float* params_f32, int obs_dim, int hidden, int act_dim
     int rc = launch_gru_bptt<NetG, MODE_FVP>(a, &grid, st);
     if (rc) return rc;
   });
-  FinArgs f{};
-  f.partial = ws; f.nblocks = grid; f.K = P; f.vec_out = Hx_out; f.tri_out = nullptr;
-  f.scale = scale; f.count = count; f.post = FIN_FVP; f.ols = ols; f.A = act_dim;
-  f.params32 = params_f32; f.log_min_std = -INFINITY; f.x = x; f.reg = reg_coeff; f.diag_scale = diag_scale;
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  return launch_finalize_update(fin_fvp(ws, grid, P, Hx_out, scale, count, {ols, act_dim, params_f32, nullptr, -INFINITY},
+                                        x, reg_coeff, diag_scale),
+                                st);
 }
 
 int b200rl_gru_update_f64(int mode, int loss_kind, const double* params_f64, int obs_dim, int hidden, int act_dim,
@@ -1057,12 +1001,8 @@ int b200rl_gru_update_f64(int mode, int loss_kind, const double* params_f64, int
                           const double* count, double reg_coeff, double diag_scale, double* vec_out, double* loss_out,
                           double* h64, double* ws, void* stream) {
   B200RL_REQUIRE(params_f64 && obs && act && tstep && h64 && ws && N > 0 && T > 0, "gru_update_f64: bad arguments");
-  B200RL_REQUIRE(mode == MODE_LOSS || mode == MODE_GRAD || mode == MODE_FVP, "gru_update_f64: bad mode");
-  B200RL_REQUIRE(mode == MODE_FVP ? (x && vec_out) : (adv && old_mean && old_log_std), "gru_update_f64: null buffer");
-  B200RL_REQUIRE(mode != MODE_GRAD || vec_out, "gru_update_f64: gradient output missing");
-  B200RL_REQUIRE(mode != MODE_LOSS || loss_out, "gru_update_f64: loss output missing");
-  B200RL_REQUIRE(loss_kind == B200RL_LOSS_TRPO || loss_kind == B200RL_LOSS_VPG ||
-                 (loss_kind == B200RL_LOSS_KL && mode == MODE_GRAD), "gru_update_f64: bad loss kind");
+  if (int rc = check_f64_args("gru_update_f64", mode, loss_kind, adv && old_mean && old_log_std, x, vec_out, loss_out))
+    return rc;
   B200RL_REQUIRE_GRU_SHAPE(obs_dim, hidden, act_dim, "gru_update_f64");
   cudaStream_t st = (cudaStream_t)stream;
   GruArgs64 a{};
@@ -1077,17 +1017,11 @@ int b200rl_gru_update_f64(int mode, int loss_kind, const double* params_f64, int
                                  : launch_gru_f64<NetG, MODE_FVP>(a, &grid, st);
     if (rc) return rc;
   });
-  FinArgs f{};
-  f.nblocks = grid; f.scale = scale; f.count = count; f.ols = ols; f.A = act_dim; f.post = FIN_NONE;
-  f.params64 = params_f64; f.log_min_std = -INFINITY;
-  if (mode != MODE_LOSS) { f.partial = ws; f.K = P; f.vec_out = vec_out; }
-  if (mode == MODE_GRAD && loss_kind != B200RL_LOSS_KL) f.post = FIN_GRAD;
-  if (mode == MODE_FVP) { f.post = FIN_FVP; f.x = x; f.reg = reg_coeff; f.diag_scale = diag_scale; }
-  if (mode != MODE_FVP && loss_out != nullptr) {
-    f.tri_partial = (mode == MODE_LOSS) ? ws : ws + (size_t)grid * P;
-    f.NT = 3; f.tri_out = loss_out;
-  }
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  // the gradient of mean KL is not masked where the min_std clamp would be active (the GRU's log_std is unclamped, and
+  // with log_min_std = -inf the mask would still zero a NaN log_std entry): no log_std block for it
+  const int A = (mode == MODE_GRAD && loss_kind == B200RL_LOSS_KL) ? 0 : act_dim;
+  return launch_finalize_update(fin_f64(mode, ws, grid, P, vec_out, loss_out, scale, count,
+                                        {ols, A, nullptr, params_f64, -INFINITY}, x, reg_coeff, diag_scale),
+                                st);
 }
 }

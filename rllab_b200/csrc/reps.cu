@@ -127,13 +127,7 @@ __global__ void __launch_bounds__(REPS_THREADS)
   block_reduce_store<K>(acc, scratch, partial + (size_t)blockIdx.x * K);
 }
 
-static int reps_grid(long long B) {
-  long long g = (B + REPS_THREADS - 1) / REPS_THREADS;
-  const long long cap = (long long)num_sms() * REPS_BLOCKS_PER_SM;
-  if (g > cap) g = cap;
-  if (g > MAX_PARTIAL_BLOCKS) g = MAX_PARTIAL_BLOCKS;
-  return (int)(g < 1 ? 1 : g);
-}
+static int reps_grid(long long B) { return partial_grid(REPS_BLOCKS_PER_SM, (B + REPS_THREADS - 1) / REPS_THREADS); }
 
 static bool reps_obs_dim_ok(int O) { return O == 2 || O == 3 || O == 4 || O == 6 || O == 13 || O == 20; }
 

@@ -16,21 +16,7 @@ constexpr int ROLLOUT_THREADS = 128;
 template <class Env, int H>
 constexpr int rollout_minblocks() { return (H == 32 && Env::S <= 4) ? 4 : 1; }
 
-struct RolloutArgs {
-  const float* params;
-  float log_min_std;
-  int N, T, max_path_length;
-  const float* eps;
-  const float* reset_raw;
-  uint32_t seed, iter;
-  long long lane0;
-  float *obs, *act, *mean, *rew;
-  unsigned char* flags;
-  unsigned short* tstep;
-  float* log_std_out;
-};
-
-// One thread per lane; the whole T-step trajectory of a lane stays in that thread's registers.
+// One thread per lane (lane_rollout, envs.cuh); the head is the Gaussian MLP policy.
 template <class Env, int H>
 __global__ void __launch_bounds__(ROLLOUT_THREADS, rollout_minblocks<Env, H>()) rollout_kernel(RolloutArgs a) {
   using N_ = Net<Env::O, H, H, Env::A>;
@@ -52,45 +38,23 @@ __global__ void __launch_bounds__(ROLLOUT_THREADS, rollout_minblocks<Env, H>()) 
   }
   if (n >= a.N) return;
   const long long lane = a.lane0 + n;
-  const size_t N = a.N, TN = (size_t)a.T * a.N;
-
-  float s[Env::S];
-  draw_reset<Env>(s, a.reset_raw, 0, a.N, n, a.seed, a.iter, lane);
-  int plen = 0;
-  for (int t = 0; t < a.T; ++t) {
-    float o[Env::O], h1[H], h2[H], mu[Env::A], e[Env::A], act[Env::A], u[Env::A];
-    // compiler barrier: without it the loop-invariant LDS of all P weights is hoisted out of the t loop and spilled
-    asm volatile("" ::: "memory");
-    Env::obs(s, o);
-    mlp_forward_thread<N_>(sp, o, h1, h2, mu, hcol, ROLLOUT_THREADS);
-    draw_eps<Env::A>(e, a.eps, t, a.N, n, a.seed, a.iter, lane);
-    const size_t idx = (size_t)t * N + n;
+  float mu[Env::A], e[Env::A];
+  lane_rollout<Env>(
+      a, n,
+      [&](int t, int, const float (&o)[Env::O]) {
+        float h1[H], h2[H];
+        mlp_forward_thread<N_>(sp, o, h1, h2, mu, hcol, ROLLOUT_THREADS);
+        draw_eps<Env::A>(e, a.eps, t, a.N, n, a.seed, a.iter, lane);
+      },
+      [&](size_t idx, size_t TN, float (&u)[Env::A]) {
 #pragma unroll
-    for (int k = 0; k < Env::O; ++k) a.obs[k * TN + idx] = o[k];
-#pragma unroll
-    for (int k = 0; k < Env::A; ++k) {
-      act[k] = fmaf(std_[k], e[k], mu[k]);  // rnd * exp(log_std) + mean   (gaussian_mlp_policy.py:129)
-      u[k] = scale_action(act[k], Env::lb(k), Env::ub(k));
-      a.act[k * TN + idx] = act[k];
-      a.mean[k * TN + idx] = mu[k];
-    }
-    float r;
-    bool done;
-    Env::step(s, u, r, done);
-    a.tstep[idx] = (unsigned short)plen;
-    ++plen;
-    const bool whole = done || (plen >= a.max_path_length);
-    const bool end = whole || (t == a.T - 1);
-    a.rew[idx] = r;
-    // FLAG_CUT: the path is cut by the end of the lane buffer, not by the env or max_path_length (process_samples drops
-    // such paths when the caller asks for whole paths only, batch_polopt.py:30-34)
-    a.flags[idx] = (unsigned char)((done ? B200RL_FLAG_DONE : 0) | (end ? B200RL_FLAG_END : 0) |
-                                   ((end && !whole) ? B200RL_FLAG_CUT : 0));
-    if (end) {
-      draw_reset<Env>(s, a.reset_raw, t + 1, a.N, n, a.seed, a.iter, lane);
-      plen = 0;
-    }
-  }
+        for (int k = 0; k < Env::A; ++k) {
+          const float act = fmaf(std_[k], e[k], mu[k]);  // rnd * exp(log_std) + mean   (gaussian_mlp_policy.py:129)
+          u[k] = scale_action(act, Env::lb(k), Env::ub(k));
+          a.act[k * TN + idx] = act;
+          a.mean[k * TN + idx] = mu[k];
+        }
+      });
 }
 
 template <class Env>
@@ -296,20 +260,12 @@ int b200rl_rollout(int env_kind, const float* params_f32, int h1, int h2, float 
                    int max_path_length, const float* eps, const float* reset_raw, unsigned int seed,
                    unsigned int iter, long long lane0, float* obs, float* act, float* mean, float* rew,
                    unsigned char* flags, unsigned short* tstep, float* log_std_out, void* stream) {
-  B200RL_REQUIRE(params_f32 && obs && act && mean && rew && flags && tstep && log_std_out, "rollout: null buffer");
-  B200RL_REQUIRE(N > 0 && T > 0 && max_path_length > 0, "rollout: N, T, max_path_length must be positive");
-  B200RL_REQUIRE(max_path_length <= 65535, "rollout: max_path_length must fit uint16 tstep");
+  const RolloutArgs a{params_f32, min_std > 0.f ? logf(min_std) : -INFINITY, N, T, max_path_length, eps, reset_raw,
+                      seed, iter, lane0, obs, act, mean, rew, flags, tstep, log_std_out};
+  if (int rc = check_rollout_args("rollout", a, true)) return rc;
   B200RL_REQUIRE(h1 == h2, "rollout: hidden sizes must be equal (32,32) or (64,64)");
   B200RL_REQUIRE(env_kind != B200RL_ENV_GYM_CARTPOLE,
                  "rollout: env kind %d has a discrete action space (b200rl_rollout_categorical drives it)", env_kind);
-  RolloutArgs a;
-  a.params = params_f32;
-  a.log_min_std = min_std > 0.f ? logf(min_std) : -INFINITY;
-  a.N = N; a.T = T; a.max_path_length = max_path_length;
-  a.eps = eps; a.reset_raw = reset_raw;
-  a.seed = seed; a.iter = iter; a.lane0 = lane0;
-  a.obs = obs; a.act = act; a.mean = mean; a.rew = rew; a.flags = flags; a.tstep = tstep;
-  a.log_std_out = log_std_out;
   B200RL_DISPATCH_ENV(env_kind, {
     int rc = launch_rollout<Env>(h1, a, (cudaStream_t)stream);
     if (rc) return rc;

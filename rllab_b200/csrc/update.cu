@@ -121,7 +121,7 @@ int b200rl_loss_kl(int loss_kind, const float* params_f32, int obs_dim, int h1, 
                    double* ws, void* stream) {
   B200RL_REQUIRE(params_f32 && obs && act && adv && old_mean && old_log_std && out && ws && B > 0,
                  "loss_kl: bad arguments");
-  B200RL_REQUIRE(loss_kind == B200RL_LOSS_TRPO || loss_kind == B200RL_LOSS_VPG, "loss_kl: bad loss kind");
+  if (int rc = check_loss_kind("loss_kl", loss_kind)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   UpdArgs a{};
   fill_args(a, params_f32, min_std, B, obs, act, adv, old_mean, old_log_std, loss_kind, flags, ws);
@@ -136,19 +136,11 @@ int b200rl_loss_kl(int loss_kind, const float* params_f32, int obs_dim, int h1, 
   } else
 #endif
   {
-    long long g = (long long)num_sms() * 4;
-    const long long need = (B + LOSS_THREADS - 1) / LOSS_THREADS;
-    if (g > need) g = need;
-    if (g > MAX_PARTIAL_BLOCKS) g = MAX_PARTIAL_BLOCKS;
-    grid = (int)g;
+    grid = partial_grid(4, (B + LOSS_THREADS - 1) / LOSS_THREADS);
     B200RL_DISPATCH_NET({ loss_thread_kernel<NetT><<<grid, LOSS_THREADS, 0, st>>>(a); });
     B200RL_LAUNCH_CHECK("loss_thread_kernel");
   }
-  FinArgs f{};
-  f.partial = nullptr; f.nblocks = grid; f.K = 0; f.vec_out = nullptr;
-  f.tri_partial = ws; f.NT = 3; f.tri_out = out; f.scale = scale; f.count = count; f.post = FIN_NONE;
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  return launch_finalize_update(fin_loss(ws, grid, out, scale, count), st);
 }
 
 int b200rl_grad(int loss_kind, const float* params_f32, int obs_dim, int h1, int h2, int act_dim, float min_std,
@@ -157,7 +149,7 @@ int b200rl_grad(int loss_kind, const float* params_f32, int obs_dim, int h1, int
                 double* loss_out, float* h_cache_out, double* ws, void* stream) {
   B200RL_REQUIRE(params_f32 && obs && act && adv && old_mean && old_log_std && g_out && ws && B > 0,
                  "grad: bad arguments");
-  B200RL_REQUIRE(loss_kind == B200RL_LOSS_TRPO || loss_kind == B200RL_LOSS_VPG, "grad: bad loss kind");
+  if (int rc = check_loss_kind("grad", loss_kind)) return rc;
   B200RL_REQUIRE(h1 == h2 && (h1 == 32 || h1 == 64), "grad: hidden sizes must be (32,32) or (64,64)");
   cudaStream_t st = (cudaStream_t)stream;
   UpdArgs a{};
@@ -175,13 +167,8 @@ int b200rl_grad(int loss_kind, const float* params_f32, int obs_dim, int h1, int
                       : update_umma64_launch(MODE_GRAD, obs_dim, act_dim, a, &grid, &P, &ols, st);
 #endif
   if (rc) return rc;
-  FinArgs f{};
-  f.partial = ws; f.nblocks = grid; f.K = P; f.vec_out = g_out;
-  f.tri_partial = ws + (size_t)grid * P; f.NT = 3; f.tri_out = loss_out;   // per-block triples follow the [grid][P] partials
-  f.scale = scale; f.count = count; f.post = FIN_GRAD; f.ols = ols; f.A = act_dim;
-  f.params32 = params_f32; f.log_min_std = (double)a.log_min_std;
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  return launch_finalize_update(
+      fin_grad(ws, grid, P, g_out, loss_out, scale, count, {ols, act_dim, params_f32, nullptr, a.log_min_std}), st);
 }
 
 int b200rl_grad_penalized(int loss_kind, double penalty, const float* params_f32, int obs_dim, int h1, int h2,
@@ -190,7 +177,7 @@ int b200rl_grad_penalized(int loss_kind, double penalty, const float* params_f32
                           const double* count, double* g_out, double* loss_out, double* ws, void* stream) {
   B200RL_REQUIRE(params_f32 && obs && act && adv && old_mean && old_log_std && g_out && ws && B > 0,
                  "grad_penalized: bad arguments");
-  B200RL_REQUIRE(loss_kind == B200RL_LOSS_TRPO || loss_kind == B200RL_LOSS_VPG, "grad_penalized: bad loss kind");
+  if (int rc = check_loss_kind("grad_penalized", loss_kind)) return rc;
   B200RL_REQUIRE(h1 == h2 && (h1 == 32 || h1 == 64), "grad_penalized: hidden sizes must be (32,32) or (64,64)");
   B200RL_REQUIRE(penalty >= 0.0 && penalty <= 3.0e38, "grad_penalized: penalty must be finite and >= 0");
 #ifdef B200RL_AB_TILE32
@@ -209,13 +196,8 @@ int b200rl_grad_penalized(int loss_kind, double penalty, const float* params_f32
   int rc = (h1 == 32) ? update_umma32_launch(mode, obs_dim, act_dim, a, &grid, &P, &ols, st)
                       : update_umma64_launch(mode, obs_dim, act_dim, a, &grid, &P, &ols, st);
   if (rc) return rc;
-  FinArgs f{};
-  f.partial = ws; f.nblocks = grid; f.K = P; f.vec_out = g_out;
-  f.tri_partial = ws + (size_t)grid * P; f.NT = 3; f.tri_out = loss_out;
-  f.scale = scale; f.count = count; f.post = FIN_GRAD; f.ols = ols; f.A = act_dim;
-  f.params32 = params_f32; f.log_min_std = (double)a.log_min_std;
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  return launch_finalize_update(
+      fin_grad(ws, grid, P, g_out, loss_out, scale, count, {ols, act_dim, params_f32, nullptr, a.log_min_std}), st);
 #endif
 }
 
@@ -242,12 +224,9 @@ int b200rl_fvp(const float* params_f32, int obs_dim, int h1, int h2, int act_dim
            : (h_cache != nullptr) ? update_umma64_launch(MODE_FVP, obs_dim, act_dim, a, &grid, &P, &ols, st)
                                   : update_gemm_launch(MODE_FVP, obs_dim, h1, act_dim, a, &grid, &P, &ols, st);
   if (rc) return rc;
-  FinArgs f{};
-  f.partial = ws; f.nblocks = grid; f.K = P; f.vec_out = Hx_out; f.tri_out = nullptr;
-  f.scale = scale; f.count = count; f.post = FIN_FVP; f.ols = ols; f.A = act_dim;
-  f.params32 = params_f32; f.log_min_std = (double)a.log_min_std; f.x = x; f.reg = reg_coeff; f.diag_scale = diag_scale;
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  return launch_finalize_update(fin_fvp(ws, grid, P, Hx_out, scale, count,
+                                        {ols, act_dim, params_f32, nullptr, a.log_min_std}, x, reg_coeff, diag_scale),
+                                st);
 }
 
 int b200rl_count_valid(long long B, const unsigned char* flags, const int* tile_list, int n_list, double* count_out,

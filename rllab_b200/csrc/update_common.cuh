@@ -5,9 +5,6 @@
 
 namespace b200rl {
 
-// MODE_GRAD_KL: MODE_GRAD plus penalty * (gradient of the per-sample KL(old || new)), the objective of the penalised
-// L-BFGS policy update (tensor-core kernels only: update_umma.cu, update_umma32.cu)
-constexpr int MODE_LOSS = 0, MODE_GRAD = 1, MODE_FVP = 2, MODE_GRAD_KL = 3;
 constexpr bool is_grad_mode(int mode) { return mode == MODE_GRAD || mode == MODE_GRAD_KL; }
 
 struct UpdArgs {

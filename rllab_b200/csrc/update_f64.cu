@@ -223,12 +223,8 @@ int b200rl_update_f64(int mode, int loss_kind, const double* params_f64, int obs
                       double scale, const double* count, double reg_coeff, double diag_scale, double* vec_out,
                       double* loss_out, double* ws, void* stream) {
   B200RL_REQUIRE(params_f64 && obs && ws && B > 0, "update_f64: bad arguments");
-  B200RL_REQUIRE(mode == MODE_LOSS || mode == MODE_GRAD || mode == MODE_FVP, "update_f64: bad mode");
-  B200RL_REQUIRE(mode == MODE_FVP ? (x && vec_out) : (act && adv && old_mean && old_log_std), "update_f64: null buffer");
-  B200RL_REQUIRE(mode != MODE_GRAD || vec_out, "update_f64: gradient output missing");
-  B200RL_REQUIRE(mode != MODE_LOSS || loss_out, "update_f64: loss output missing");
-  B200RL_REQUIRE(loss_kind == B200RL_LOSS_TRPO || loss_kind == B200RL_LOSS_VPG ||
-                 (loss_kind == B200RL_LOSS_KL && mode == MODE_GRAD), "update_f64: bad loss kind");
+  if (int rc = check_f64_args("update_f64", mode, loss_kind, act && adv && old_mean && old_log_std, x, vec_out, loss_out))
+    return rc;
   cudaStream_t st = (cudaStream_t)stream;
   UpdArgs64 a{};
   a.params = params_f64; a.xvec = x; a.log_min_std = min_std > 0.0 ? log(min_std) : -INFINITY; a.B = B;
@@ -242,17 +238,8 @@ int b200rl_update_f64(int mode, int loss_kind, const double* params_f64, int obs
                                  : launch_f64<NetT, MODE_FVP>(a, &grid, st);
     if (rc) return rc;
   });
-  FinArgs f{};
-  f.nblocks = grid; f.scale = scale; f.count = count; f.ols = ols; f.A = act_dim;
-  f.params64 = params_f64; f.log_min_std = a.log_min_std;
-  if (mode != MODE_LOSS) { f.partial = ws; f.K = P; f.vec_out = vec_out; }
-  f.post = (mode == MODE_GRAD) ? FIN_GRAD : (mode == MODE_FVP ? FIN_FVP : FIN_NONE);
-  if (mode == MODE_FVP) { f.x = x; f.reg = reg_coeff; f.diag_scale = diag_scale; }
-  if (mode != MODE_FVP && loss_out != nullptr) {
-    f.tri_partial = (mode == MODE_LOSS) ? ws : ws + (size_t)grid * P;
-    f.NT = 3; f.tri_out = loss_out;
-  }
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  return launch_finalize_update(fin_f64(mode, ws, grid, P, vec_out, loss_out, scale, count,
+                                        {ols, act_dim, nullptr, params_f64, a.log_min_std}, x, reg_coeff, diag_scale),
+                                st);
 }
 }

@@ -123,21 +123,17 @@ __global__ void vf_stats_finish_kernel(const double* __restrict__ acc, double* _
 template <int O>
 static int vf_norm_stats_run(long long B, const float* obs, const float* y, const unsigned char* flags, int stage,
                              double* acc, double* stats, double* ws, cudaStream_t st) {
-  long long g = (long long)num_sms() * 4;
-  const long long need = (B + VF_STATS_THREADS - 1) / VF_STATS_THREADS;
-  if (g > need) g = need;
-  if (g > MAX_PARTIAL_BLOCKS) g = MAX_PARTIAL_BLOCKS;
-  if (g < 1) g = 1;
+  const int g = partial_grid(4, (B + VF_STATS_THREADS - 1) / VF_STATS_THREADS);
   if (stage == 0 || stage == 3) {
-    vf_stats_kernel<O, 0><<<(unsigned)g, VF_STATS_THREADS, 0, st>>>(B, obs, y, flags, acc, ws);
+    vf_stats_kernel<O, 0><<<g, VF_STATS_THREADS, 0, st>>>(B, obs, y, flags, acc, ws);
     B200RL_LAUNCH_CHECK("vf_stats_kernel<0>");
-    int rc = launch_finalize_sum(ws, (int)g, O + 2, acc, 1.0, st);
+    int rc = launch_finalize_sum(ws, g, O + 2, acc, 1.0, st);
     if (rc) return rc;
   }
   if (stage == 1 || stage == 3) {
-    vf_stats_kernel<O, 1><<<(unsigned)g, VF_STATS_THREADS, 0, st>>>(B, obs, y, flags, acc, ws);
+    vf_stats_kernel<O, 1><<<g, VF_STATS_THREADS, 0, st>>>(B, obs, y, flags, acc, ws);
     B200RL_LAUNCH_CHECK("vf_stats_kernel<1>");
-    int rc = launch_finalize_sum(ws, (int)g, O + 1, acc + O + 2, 1.0, st);
+    int rc = launch_finalize_sum(ws, g, O + 1, acc + O + 2, 1.0, st);
     if (rc) return rc;
   }
   if (stage == 2 || stage == 3) {
@@ -321,14 +317,10 @@ static int vf_launch_loss_grad(const VfArgs& a, int* grid_out, cudaStream_t st) 
   int per_sm = (int)((228 * 1024) / (SM::bytes + 1024));
   if (per_sm < 1) per_sm = 1;
   if (per_sm > 2) per_sm = 2;
-  long long grid = (long long)num_sms() * per_sm;
-  const long long ntiles = (a.B + VF_TILE - 1) / VF_TILE;
-  if (grid > ntiles) grid = ntiles;
-  if (grid > MAX_PARTIAL_BLOCKS) grid = MAX_PARTIAL_BLOCKS;
-  if (grid < 1) grid = 1;
-  vf_loss_grad_kernel<N, GRAD><<<(unsigned)grid, VF_THREADS, SM::bytes, st>>>(a);
+  const int grid = partial_grid(per_sm, (a.B + VF_TILE - 1) / VF_TILE);
+  vf_loss_grad_kernel<N, GRAD><<<grid, VF_THREADS, SM::bytes, st>>>(a);
   B200RL_LAUNCH_CHECK("vf_loss_grad_kernel");
-  *grid_out = (int)grid;
+  *grid_out = grid;
   return 0;
 }
 
@@ -405,12 +397,8 @@ int b200rl_vf_loss_grad(const float* params_f32, int obs_dim, int h1, int h2, lo
     int rc = g_out ? vf_launch_loss_grad<NetT, true>(a, &grid, st) : vf_launch_loss_grad<NetT, false>(a, &grid, st);
     if (rc) return rc;
   });
-  FinArgs f{};
-  f.partial = ws; f.nblocks = grid; f.K = g_out ? P : 0; f.vec_out = g_out;
-  f.tri_partial = ws + (g_out ? (size_t)grid * P : 0); f.NT = 3; f.tri_out = loss_out;
-  f.scale = scale; f.count = count; f.post = FIN_NONE;
-  if (peer_fused()) f.peer = peer_next();
-  return launch_finalize_update(f, st);
+  // the regressor has no log_std block: the gradient's min_std mask touches no entry
+  return launch_finalize_update(fin_grad(ws, grid, g_out ? P : 0, g_out, loss_out, scale, count, {}), st);
 }
 
 }  // extern "C"
