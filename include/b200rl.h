@@ -363,6 +363,69 @@ int b200rl_gru_update_f64(int mode, int loss_kind, const double* params_f64, int
                           const double* count, double reg_coeff, double diag_scale, double* vec_out, double* loss_out,
                           double* h64, double* ws, void* stream);
 
+/* ---- CategoricalGRUPolicy (rllab/policies/categorical_gru_policy.py, rllab/core/network.py GRUNetwork with a softmax
+ * output, rllab/distributions/recurrent_categorical.py).  The GaussianGRUPolicy cell above with x_t = [obs_t, one-hot
+ * prev_action_t] (include_action != 0) or obs_t, logits z = h' W_out + b_out and prob = softmax(z); no log_std.  Flat
+ * layout [W_xr, W_hr, b_r, W_xu, W_hu, b_u, W_xc, W_hc, b_c, W_out (H x n), b_out (n)].  h = 0 and prev_action = 0 at a
+ * path start; inside a path prev_action is the previous one-hot action act[t-1].  Compiled for obs_dim 4, hidden 32,
+ * n_actions 2 (CartPole-v0), either include_action; other shapes return B200RL_EUNSUPPORTED.  The entry points mirror
+ * the b200rl_gru_* ones with the categorical conventions of b200rl_categorical_*: act [n][T][N] one-hot, old_prob
+ * [n][T][N] in place of old_mean / old_log_std, the 1e-8 of categorical.py in the ratio and the KL, and a Fisher-vector
+ * product J^T M J x with M the full n x n logit block at theta_old. ---- */
+long long b200rl_categorical_gru_num_params(int obs_dim, int hidden, int n_actions, int include_action);
+
+/* One GRU step for n rows (CategoricalGRUPolicy.get_action, vectorised): obs [O][n], prev_action [n_actions][n] one-hot
+ * (NULL = 0), h_in [H][n] (NULL = 0) -> act_out [n] int32 = weighted_sample(prob, u), prob_out [n_actions][n], h_out
+ * [H][n].  u [n] or NULL (Philox stream 0 at (lane0 + i, row), as b200rl_categorical_get_actions). */
+int b200rl_categorical_gru_get_actions(const float* params_f32, int obs_dim, int hidden, int n_actions,
+                                       int include_action, const float* obs, const float* prev_action,
+                                       const float* h_in, long long n, const float* u, unsigned int seed,
+                                       unsigned int iter, int row, long long lane0, int* act_out, float* prob_out,
+                                       float* h_out, void* stream);
+
+/* Fused rollout with the categorical GRU policy: b200rl_rollout_categorical's planes (obs, one-hot act, prob, rew, flags,
+ * tstep) and action draw (u [T][N] or NULL = Philox stream 0 row t), with h and prev_action carried per lane and reset at
+ * every path start. */
+int b200rl_rollout_categorical_gru(int env_kind, const float* params_f32, int hidden, int include_action, int N, int T,
+                                   int max_path_length, const float* u, const float* reset_raw, unsigned int seed,
+                                   unsigned int iter, long long lane0, float* obs, float* act, float* prob, float* rew,
+                                   unsigned char* flags, unsigned short* tstep, void* stream);
+
+/* (loss, sum KL, max KL) as b200rl_gru_loss_kl with the losses of b200rl_categorical_loss_kl. */
+int b200rl_categorical_gru_loss_kl(int loss_kind, const float* params_f32, int obs_dim, int hidden, int n_actions,
+                                   int include_action, int N, int T, const float* obs, const float* act,
+                                   const unsigned short* tstep, const float* adv, const float* old_prob,
+                                   const unsigned char* flags, double scale, const double* count, double* out,
+                                   float* h_cache_out, double* ws, void* stream);
+
+/* Backpropagation-through-time gradient of the surrogate plus penalty * mean KL, as b200rl_gru_grad. */
+int b200rl_categorical_gru_grad(int loss_kind, double penalty, const float* params_f32, int obs_dim, int hidden,
+                                int n_actions, int include_action, int N, int T, const float* obs, const float* act,
+                                const unsigned short* tstep, const float* adv, const float* old_prob,
+                                const unsigned char* flags, double scale, const double* count, double* g_out,
+                                double* loss_out, float* h_cache, double* ws, void* stream);
+
+/* Fisher-vector product J^T M J x (+ diag_scale * reg_coeff * x) at theta_old, as b200rl_gru_fvp: the forward tangent
+ * sweep writes M(p_old) J x per sample into plane [n_actions][T][N] (float32 scratch of the caller, so any batch that
+ * fits in memory runs), then the backward sweep reads it (M as in b200rl_categorical_fvp, the O(1e-8) first-derivative
+ * term left out). */
+int b200rl_categorical_gru_fvp(const float* params_f32, int obs_dim, int hidden, int n_actions, int include_action,
+                               int N, int T, const float* obs, const float* act, const unsigned short* tstep,
+                               const unsigned char* flags, const double* x, double scale, const double* count,
+                               double reg_coeff, double diag_scale, double* Hx_out, float* h_cache, int h_valid,
+                               float* plane, double* ws, void* stream);
+
+/* float64 parity mode, as b200rl_gru_update_f64 (mode 0 loss/KL, 1 gradient, B200RL_LOSS_KL with mode 1 the gradient
+ * of mean KL for FiniteDifferenceHvp, 2 Fisher-vector product).  h64 [H + n][T][N] float64 scratch.  Mode 2 is the
+ * Gauss-Newton product J^T M J x of the float32 pass in float64: unlike b200rl_categorical_update_f64 it leaves out the
+ * O(1e-8) first-derivative term as well (DESIGN.md section 5). */
+int b200rl_categorical_gru_update_f64(int mode, int loss_kind, const double* params_f64, int obs_dim, int hidden,
+                                      int n_actions, int include_action, int N, int T, const float* obs,
+                                      const float* act, const unsigned short* tstep, const float* adv,
+                                      const float* old_prob, const unsigned char* flags, const double* x, double scale,
+                                      const double* count, double reg_coeff, double diag_scale, double* vec_out,
+                                      double* loss_out, double* h64, double* ws, void* stream);
+
 /* ---- GaussianMLPRegressor, the value function of GaussianMLPBaseline (rllab/regressors/gaussian_mlp_regressor.py,
  * rllab/baselines/gaussian_mlp_baseline.py).  Net: MLP(obs_dim -> h1 -> h2 -> 1), ReLU hidden units, no output
  * nonlinearity, one state-independent log_std (rllab/core/network.py:36-81, lasagne_layers.py ParamLayer); the flat

@@ -121,6 +121,19 @@ SIGNATURES = {
                                c_double, _P, _P, c_int, _P, _P]),
     "b200rl_gru_update_f64": (c_int, [c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P,
                                       _P, _P, _P, c_double, _P, c_double, c_double, _P, _P, _P, _P, _P]),
+    "b200rl_categorical_gru_num_params": (_LL, [c_int, c_int, c_int, c_int]),
+    "b200rl_categorical_gru_get_actions": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _LL, _P, c_uint, c_uint,
+                                                   c_int, _LL, _P, _P, _P, _P]),
+    "b200rl_rollout_categorical_gru": (c_int, [c_int, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_uint, c_uint, _LL,
+                                               _P, _P, _P, _P, _P, _P, _P]),
+    "b200rl_categorical_gru_loss_kl": (c_int, [c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P,
+                                               _P, c_double, _P, _P, _P, _P, _P]),
+    "b200rl_categorical_gru_grad": (c_int, [c_int, c_double, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P,
+                                            _P, _P, _P, c_double, _P, _P, _P, _P, _P, _P]),
+    "b200rl_categorical_gru_fvp": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_double,
+                                           _P, c_double, c_double, _P, _P, c_int, _P, _P, _P]),
+    "b200rl_categorical_gru_update_f64": (c_int, [c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P,
+                                                  _P, _P, _P, _P, c_double, _P, c_double, c_double, _P, _P, _P, _P, _P]),
 }
 
 _lib = None
@@ -218,4 +231,11 @@ def gru_num_params(O, H, A, include_action):
     p = load().b200rl_gru_num_params(O, H, A, int(bool(include_action)))
     if p < 0:
         raise B200RLError("unsupported GRU network O=%d hidden=%d A=%d: %s" % (O, H, A, last_error()))
+    return int(p)
+
+
+def categorical_gru_num_params(O, H, n, include_action):
+    p = load().b200rl_categorical_gru_num_params(O, H, n, int(bool(include_action)))
+    if p < 0:
+        raise B200RLError("unsupported categorical GRU network O=%d hidden=%d n=%d: %s" % (O, H, n, last_error()))
     return int(p)

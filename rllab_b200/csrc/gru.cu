@@ -21,6 +21,7 @@
 // tile, float32 inside the tile and float64 across tiles, each entry owned by one thread (fixed order, no atomics).
 // Per-block partials go through launch_finalize_update, so the min_std mask, the log_std block of the Fisher product and
 // the fused peer exchange are the Gaussian passes'.
+#include "cat_head.cuh"
 #include "envs.cuh"
 #include "update_common.cuh"
 
@@ -30,6 +31,7 @@ constexpr int GRU_H = 32;
 
 template <int O_, int A_, int INC>
 struct GruNet {
+  static constexpr bool CAT = false;   // Gaussian head: linear mean, log_std
   static constexpr int O = O_, A = A_, H = GRU_H, I = O_ + (INC ? A_ : 0);
   static constexpr int G = I * H + H * H + H;   // one gate block: W_x, W_h, b
   static constexpr int oWo = 3 * G, obo = oWo + H * A, ols = obo + A, P = ols + A, P4 = (P + 3) & ~3;
@@ -38,7 +40,32 @@ struct GruNet {
   __host__ __device__ static constexpr int ob(int g) { return g * G + I * H + H * H; }
 };
 
+// CategoricalGRUPolicy's net: the same cell and W_out / b_out, whose A = n outputs are the logits of a softmax; no log_std
+// (P = ols).  The update passes branch on N::CAT where the heads differ.
+template <int O_, int NA, int INC>
+struct GruCatNet : GruNet<O_, NA, INC> {
+  static constexpr bool CAT = true;
+  static constexpr int P = GruNet<O_, NA, INC>::ols, P4 = (P + 3) & ~3;
+};
+
 inline bool gru_supported(int O, int H, int A) { return O == 4 && H == GRU_H && A == 1; }
+inline bool gru_cat_supported(int O, int H, int n) { return O == 4 && H == GRU_H && n == 2; }
+#define B200RL_REQUIRE_GRU_CAT_SHAPE(O_, H_, n_, what)                                                              \
+  do {                                                                                                              \
+    if (!gru_cat_supported(O_, H_, n_)) {                                                                           \
+      set_error("%s: categorical GRU net obs_dim=%d hidden=%d n=%d is not compiled in (only obs 4, hidden 32, n 2)", \
+                what, (int)(O_), (int)(H_), (int)(n_));                                                             \
+      return B200RL_EUNSUPPORTED;                                                                                   \
+    }                                                                                                               \
+  } while (0)
+#define B200RL_DISPATCH_GRU_CAT(inc, ...)                \
+  if (inc) {                                            \
+    using NetG = ::b200rl::GruCatNet<4, 2, 1>;          \
+    __VA_ARGS__;                                        \
+  } else {                                              \
+    using NetG = ::b200rl::GruCatNet<4, 2, 0>;          \
+    __VA_ARGS__;                                        \
+  }
 #define B200RL_REQUIRE_GRU_SHAPE(O_, H_, A_, what)                                                                 \
   do {                                                                                                             \
     if (!gru_supported(O_, H_, A_)) {                                                                              \
@@ -202,6 +229,86 @@ __global__ void __launch_bounds__(128) gru_get_actions_kernel(const float* __res
   for (int j = 0; j < H; ++j) h_out[(size_t)j * n_ + n] = hn[j];
 }
 
+// CategoricalGRUPolicy: action = weighted_sample(softmax(z), u) with u from a.eps [T][N] or Philox stream 0 row t (the
+// categorical rollout's draw, cat_draw_u).  act holds the one-hot action and the mean plane the probabilities; the one-hot
+// action is the next step's prev_action input.
+template <class Env, class N_>
+__global__ void __launch_bounds__(128) gru_cat_rollout_kernel(RolloutArgs a) {
+  static_assert(N_::CAT && Env::O == N_::O && EnvNumActions<Env>::value == N_::A, "env and categorical GRU net disagree");
+  constexpr int H = N_::H, A = N_::A;
+  __shared__ __align__(16) float sp[N_::P4];
+  for (int i = threadIdx.x; i < N_::P; i += blockDim.x) sp[i] = a.params[i];
+  __syncthreads();
+  const int n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= a.N) return;
+  const long long lane = a.lane0 + n;
+  float h[H], pa[A], hn[H], p[A];
+  int k_act;
+  lane_rollout<Env>(
+      a, n,
+      [&](int t, int plen, const float (&o)[Env::O]) {
+        if (plen == 0) {   // path start: h_0 = 0, prev_action = 0
+#pragma unroll
+          for (int j = 0; j < H; ++j) h[j] = 0.f;
+#pragma unroll
+          for (int k = 0; k < A; ++k) pa[k] = 0.f;
+        }
+        float x[N_::I], z[A];
+#pragma unroll
+        for (int k = 0; k < Env::O; ++k) x[k] = o[k];
+#pragma unroll
+        for (int k = 0; k < N_::I - N_::O; ++k) x[N_::O + k] = pa[k];
+        gru_cell<N_>(sp, x, h, hn);
+        gru_mean<N_>(sp, hn, z);
+        cat_softmax(z, p);
+        k_act = cat_sample(p, cat_draw_u(a.eps, t, a.N, n, a.seed, a.iter, lane));
+      },
+      [&](size_t idx, size_t TN, float (&u)[Env::A]) {
+#pragma unroll
+        for (int k = 0; k < A; ++k) {
+          pa[k] = (k == k_act) ? 1.0f : 0.0f;
+          a.act[k * TN + idx] = pa[k];
+          a.mean[k * TN + idx] = p[k];
+        }
+        u[0] = (float)k_act;
+#pragma unroll
+        for (int j = 0; j < H; ++j) h[j] = hn[j];
+      });
+}
+
+template <class N_>
+__global__ void __launch_bounds__(128) gru_cat_get_actions_kernel(const float* __restrict__ params,
+                                                                  const float* __restrict__ obs,
+                                                                  const float* __restrict__ prev_action,
+                                                                  const float* __restrict__ h_in, long long n_,
+                                                                  const float* __restrict__ u, uint32_t seed,
+                                                                  uint32_t iter, int row, long long lane0,
+                                                                  int* __restrict__ act_out, float* __restrict__ prob_out,
+                                                                  float* __restrict__ h_out) {
+  constexpr int H = N_::H, A = N_::A;
+  __shared__ __align__(16) float sp[N_::P4];
+  for (int i = threadIdx.x; i < N_::P; i += blockDim.x) sp[i] = params[i];
+  __syncthreads();
+  const long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= n_) return;
+  float x[N_::I], h[H], hn[H], z[A], p[A];
+#pragma unroll
+  for (int k = 0; k < N_::O; ++k) x[k] = obs[(size_t)k * n_ + n];
+#pragma unroll
+  for (int k = 0; k < N_::I - N_::O; ++k) x[N_::O + k] = prev_action ? prev_action[(size_t)k * n_ + n] : 0.f;
+#pragma unroll
+  for (int j = 0; j < H; ++j) h[j] = h_in ? h_in[(size_t)j * n_ + n] : 0.f;
+  gru_cell<N_>(sp, x, h, hn);
+  gru_mean<N_>(sp, hn, z);
+  cat_softmax(z, p);
+  const float uu = (u != nullptr) ? u[n] : cat_draw_u(nullptr, row, n_, n, seed, iter, lane0 + n);
+  act_out[n] = cat_sample(p, uu);
+#pragma unroll
+  for (int k = 0; k < A; ++k) prob_out[(size_t)k * n_ + n] = p[k];
+#pragma unroll
+  for (int j = 0; j < H; ++j) h_out[(size_t)j * n_ + n] = hn[j];
+}
+
 // ------------------------------------------------------------------------------------------------ per-sample terms
 struct GruArgs {
   const float* params;
@@ -211,7 +318,7 @@ struct GruArgs {
   float* plane;               // FVP: [A][T][N] scratch, M * (J x) per sample
   int N, T;
   long long B;
-  const float *obs, *act, *adv, *old_mean, *old_log_std;
+  const float *obs, *act, *adv, *old_mean, *old_log_std;   // categorical head: old_mean = old prob [n][B]
   const unsigned short* tstep;
   int loss_kind;
   float penalty;
@@ -282,6 +389,46 @@ __device__ __forceinline__ void gru_terms(const GruArgs& a, const GruDist<A>& D,
   }
 }
 
+// Categorical head (cat_head.cuh, as cat_phase_a): prob = softmax(z), the surrogate term and KL of the sample, and
+// dz = d (term + penalty * kl) / dz.
+template <int NA>
+__device__ __forceinline__ void gru_cat_terms(const GruArgs& a, size_t idx, const float (&z)[NA], float& term, float& kl,
+                                              float (&dz)[NA]) {
+  float p[NA], xa[NA], q[NA];
+  cat_softmax(z, p);
+#pragma unroll
+  for (int k = 0; k < NA; ++k) {
+    xa[k] = a.act[(size_t)k * a.B + idx];
+    q[k] = a.old_mean[(size_t)k * a.B + idx];
+  }
+  float pa, c;
+  cat_terms(a.loss_kind, p, xa, q, a.adv[idx], pa, term, kl, c);
+  cat_surr_logit_grad(c, p, xa, dz);
+  if (a.penalty > 0.f) {
+    float r[NA], g[NA];
+#pragma unroll
+    for (int k = 0; k < NA; ++k) r[k] = q[k] * p[k] / (p[k] + CAT_TINY);
+    cat_kl_logit_grad(p, r, g);
+#pragma unroll
+    for (int k = 0; k < NA; ++k) dz[k] = fmaf(a.penalty, g[k], dz[k]);
+  }
+}
+
+// The head of net N_ on the output row mu (mean or logits): the term, KL and output deltas of one sample (dls: the
+// log_std deltas, zero for the categorical head, which has no log_std)
+template <class N_>
+__device__ __forceinline__ void gru_head_terms(const GruArgs& a, const GruDist<N_::A>& D, size_t idx,
+                                               const float (&mu)[N_::A], float& term, float& kl, float (&dmu)[N_::A],
+                                               float (&dls)[N_::A]) {
+  if constexpr (N_::CAT) {
+    gru_cat_terms<N_::A>(a, idx, mu, term, kl, dmu);
+#pragma unroll
+    for (int k = 0; k < N_::A; ++k) dls[k] = 0.f;
+  } else {
+    gru_terms<N_::A>(a, D, idx, mu, term, kl, dmu, dls);
+  }
+}
+
 __device__ __forceinline__ bool gru_masked(const GruArgs& a, size_t idx) {
   return a.flags != nullptr && (a.flags[idx] & B200RL_FLAG_MASKED);
 }
@@ -296,7 +443,7 @@ __global__ void __launch_bounds__(128) gru_loss_kernel(GruArgs a) {
   for (int i = threadIdx.x; i < N_::P; i += blockDim.x) sp[i] = a.params[i];
   __syncthreads();
   GruDist<A> D;
-  D.init(sp + N_::ols, a.old_log_std);
+  if constexpr (!N_::CAT) D.init(sp + N_::ols, a.old_log_std);
   double s_loss = 0.0, s_kl = 0.0, m_kl = -1.0e300;
   const int stride = gridDim.x * blockDim.x;
   for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < a.N; n += stride) {
@@ -320,7 +467,7 @@ __global__ void __launch_bounds__(128) gru_loss_kernel(GruArgs a) {
       }
       if (gru_masked(a, idx)) continue;
       float term, kl, dmu[A], dls[A];
-      gru_terms<A>(a, D, idx, mu, term, kl, dmu, dls);
+      gru_head_terms<N_>(a, D, idx, mu, term, kl, dmu, dls);
       s_loss += (double)term;
       s_kl += (double)kl;
       m_kl = fmax(m_kl, (double)kl);
@@ -339,7 +486,7 @@ template <class N_>
 struct GruStage {
   static constexpr int I = N_::I, H = N_::H, A = N_::A;
   static constexpr int rX = 0, rHp = rX + I, rOne = rHp + H, rD = rOne + 1 /* Dr, Du, Dc */, rDhc = rD + 3 * H,
-                       rHn = rDhc + H, rDM = rHn + H, rDL = rDM + A, R = rDL + A;
+                       rHn = rDhc + H, rDM = rHn + H, rDL = rDM + A, R = rDL + (N_::CAT ? 0 : A);   // no log_std rows
   static constexpr int o_sp = 0, o_sv = N_::P4, o_stage = 2 * N_::P4;
   static constexpr int acc_off = (((o_stage + R * GLD) * 4 + 15) / 16) * 16;   // bytes
   static constexpr int red_off = acc_off + N_::P * 8;
@@ -427,13 +574,24 @@ __device__ __forceinline__ void gru_forward_lane(const GruArgs& a, const float* 
         for (int j = 0; j < H; ++j) a.hbuf[(size_t)j * a.B + idx] = hn[j];
       }
       const bool valid = !gru_masked(a, idx);
+      float md[A];
 #pragma unroll
       for (int k = 0; k < A; ++k) {
-        float md = sv[N_::obo + k];
+        md[k] = sv[N_::obo + k];
 #pragma unroll
         for (int j = 0; j < H; ++j)
-          md = fmaf(tn[j], sp[N_::oWo + j * A + k], fmaf(hn[j], sv[N_::oWo + j * A + k], md));
-        a.plane[(size_t)k * a.B + idx] = valid ? md * D.Mmu[k] : 0.f;
+          md[k] = fmaf(tn[j], sp[N_::oWo + j * A + k], fmaf(hn[j], sv[N_::oWo + j * A + k], md[k]));
+      }
+      if constexpr (N_::CAT) {   // M (J x) with the full n x n logit Fisher block at p(theta_old)
+        float z[A], p[A], m[A];
+        gru_mean<N_>(sp, hn, z);
+        cat_softmax(z, p);
+        cat_logit_hvp(p, md, m);
+#pragma unroll
+        for (int k = 0; k < A; ++k) a.plane[(size_t)k * a.B + idx] = valid ? m[k] : 0.f;
+      } else {
+#pragma unroll
+        for (int k = 0; k < A; ++k) a.plane[(size_t)k * a.B + idx] = valid ? md[k] * D.Mmu[k] : 0.f;
       }
 #pragma unroll
       for (int j = 0; j < H; ++j) { h[j] = hn[j]; th[j] = tn[j]; }
@@ -447,7 +605,7 @@ __device__ __forceinline__ void gru_forward_lane(const GruArgs& a, const float* 
       if (gru_masked(a, idx)) continue;
       float mu[A], term, kl, dmu[A], dls[A];
       gru_mean<N_>(sp, hn, mu);
-      gru_terms<A>(a, D, idx, mu, term, kl, dmu, dls);
+      gru_head_terms<N_>(a, D, idx, mu, term, kl, dmu, dls);
       s_loss += (double)term;
       s_kl += (double)kl;
       m_kl = fmax(m_kl, (double)kl);
@@ -490,7 +648,7 @@ __device__ __forceinline__ void gru_backward_step(const GruArgs& a, const float*
     if (valid) {
       float mu[A], term, kl;
       gru_mean<N_>(sp, ht, mu);
-      gru_terms<A>(a, D, idx, mu, term, kl, dmu, dls);
+      gru_head_terms<N_>(a, D, idx, mu, term, kl, dmu, dls);
     } else {
 #pragma unroll
       for (int k = 0; k < A; ++k) { dmu[k] = 0.f; dls[k] = 0.f; }
@@ -503,7 +661,7 @@ __device__ __forceinline__ void gru_backward_step(const GruArgs& a, const float*
 #pragma unroll
   for (int k = 0; k < A; ++k) {
     col[(S::rDM + k) * GLD] = dmu[k];
-    col[(S::rDL + k) * GLD] = dls[k];
+    if constexpr (!N_::CAT) col[(S::rDL + k) * GLD] = dls[k];
   }
   float dprev[H];
 #pragma unroll
@@ -570,7 +728,7 @@ __global__ void __launch_bounds__(GT, 1) gru_bptt_kernel(GruArgs a) {
   }
   __syncthreads();
   GruDist<N_::A> D;
-  D.init(sp + N_::ols, MODE == MODE_FVP ? nullptr : a.old_log_std);
+  if constexpr (!N_::CAT) D.init(sp + N_::ols, MODE == MODE_FVP ? nullptr : a.old_log_std);
   double s_loss = 0.0, s_kl = 0.0, m_kl = -1.0e300;
   const int ntiles = (a.N + GT - 1) / GT;
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -668,6 +826,53 @@ __device__ __forceinline__ void gru_input_d(const GruArgs64& a, size_t idx, bool
   for (int k = 0; k < N_::I - N_::O; ++k) x[N_::O + k] = start ? 0.0 : (double)a.act[(size_t)k * a.B + idx - a.N];
 }
 
+// Categorical head in float64 at h (the role of cat_f64_kernel's per-sample block): prob p = softmax(h W_out + b_out)
+template <class N_>
+__device__ __forceinline__ void gru_cat_prob_d(const double* sp, const double (&h)[N_::H], double (&p)[N_::A]) {
+  constexpr int H = N_::H, A = N_::A;
+  double z[A], zm = -1.0e300, es = 0.0;
+  for (int k = 0; k < A; ++k) {
+    double m = sp[N_::obo + k];
+    for (int j = 0; j < H; ++j) m = fma(h[j], sp[N_::oWo + j * A + k], m);
+    z[k] = m;
+    zm = fmax(zm, m);
+  }
+  for (int k = 0; k < A; ++k) { p[k] = exp(z[k] - zm); es += p[k]; }
+  for (int k = 0; k < A; ++k) p[k] /= es;
+}
+
+// ... and the sample's surrogate term and KL, and the logit gradient of the term (B200RL_LOSS_KL: of the KL)
+template <class N_>
+__device__ __forceinline__ void gru_cat_d(const GruArgs64& a, const double* sp, const double (&h)[N_::H], size_t idx,
+                                          double (&p)[N_::A], double& term, double& kl, double (&dz)[N_::A]) {
+  constexpr int A = N_::A;
+  constexpr double E = 1e-8;
+  gru_cat_prob_d<N_>(sp, h, p);
+  double xa[A], q[A], r[A], pa = 0.0, qa = 0.0;
+  kl = 0.0;
+  for (int k = 0; k < A; ++k) {
+    xa[k] = (double)a.act[(size_t)k * a.B + idx];
+    q[k] = (double)a.old_mean[(size_t)k * a.B + idx];
+    pa += p[k] * xa[k];
+    qa += q[k] * xa[k];
+    kl += q[k] * (log(q[k] + E) - log(p[k] + E));
+    r[k] = q[k] * p[k] / (p[k] + E);
+  }
+  const double adv_s = (double)a.adv[idx];
+  double c;
+  if (a.loss_kind == B200RL_LOSS_TRPO) {
+    term = -(pa + E) / (qa + E) * adv_s;
+    c = adv_s / (qa + E);
+  } else {
+    term = -log(pa + E) * adv_s;
+    c = adv_s / (pa + E);
+  }
+  if (a.loss_kind == B200RL_LOSS_KL)
+    cat_kl_logit_grad(p, r, dz);
+  else
+    cat_surr_logit_grad(c, p, xa, dz);
+}
+
 template <class N_, int MODE>
 __global__ void __launch_bounds__(64) gru_f64_kernel(GruArgs64 a) {
   constexpr int H = N_::H, A = N_::A, I = N_::I, P = N_::P;
@@ -683,7 +888,7 @@ __global__ void __launch_bounds__(64) gru_f64_kernel(GruArgs64 a) {
   }
   __syncthreads();
   double ls_new[A], var_new[A], var_new2[A], ls_old[A], var_old[A], sum_ls_new = 0.0, sum_ls_old = 0.0;
-  for (int k = 0; k < A; ++k) {
+  for (int k = 0; k < (N_::CAT ? 0 : A); ++k) {
     ls_new[k] = sp[N_::ols + k];
     var_new[k] = exp(2.0 * ls_new[k]);
     var_new2[k] = 2.0 * var_new[k] + 1e-8;
@@ -733,14 +938,30 @@ __global__ void __launch_bounds__(64) gru_f64_kernel(GruArgs64 a) {
       }
       const bool valid = !(a.flags != nullptr && (a.flags[idx] & B200RL_FLAG_MASKED));
       if (MODE == MODE_FVP) {
+        double md[A];
         for (int k = 0; k < A; ++k) {
-          double md = sv[N_::obo + k];
-          for (int j = 0; j < H; ++j) md += th[j] * sp[N_::oWo + j * A + k] + h[j] * sv[N_::oWo + j * A + k];
-          a.h64[(size_t)(H + k) * a.B + idx] = valid ? md * 2.0 / var_new2[k] : 0.0;
+          md[k] = sv[N_::obo + k];
+          for (int j = 0; j < H; ++j) md[k] += th[j] * sp[N_::oWo + j * A + k] + h[j] * sv[N_::oWo + j * A + k];
+        }
+        if constexpr (N_::CAT) {   // M (J x), M the logit Fisher block at p(theta_old)
+          double p[A], m[A];
+          gru_cat_prob_d<N_>(sp, h, p);
+          cat_logit_hvp(p, md, m);
+          for (int k = 0; k < A; ++k) a.h64[(size_t)(H + k) * a.B + idx] = valid ? m[k] : 0.0;
+        } else {
+          for (int k = 0; k < A; ++k) a.h64[(size_t)(H + k) * a.B + idx] = valid ? md[k] * 2.0 / var_new2[k] : 0.0;
         }
         continue;
       }
       if (!valid) continue;
+      if constexpr (N_::CAT) {
+        double p[A], term, kl, dz[A];
+        gru_cat_d<N_>(a, sp, h, idx, p, term, kl, dz);
+        s_loss += term;
+        s_kl += kl;
+        m_kl = fmax(m_kl, kl);
+        continue;
+      }
       double zsq = 0.0, zsq_old = 0.0, kl = 0.0;
       for (int k = 0; k < A; ++k) {
         double mu = sp[N_::obo + k];
@@ -773,39 +994,49 @@ __global__ void __launch_bounds__(64) gru_f64_kernel(GruArgs64 a) {
         hp[j] = start ? 0.0 : a.h64[(size_t)j * a.B + idx - a.N];
         ht[j] = a.h64[(size_t)j * a.B + idx];
       }
-      for (int k = 0; k < A; ++k) {
-        dmu[k] = 0.0;
-        dls[k] = 0.0;
-        if (!valid) continue;
-        if (MODE == MODE_FVP) { dmu[k] = a.h64[(size_t)(H + k) * a.B + idx]; continue; }
-        double mu = sp[N_::obo + k];
-        for (int j = 0; j < H; ++j) mu = fma(ht[j], sp[N_::oWo + j * A + k], mu);
-        const double act = a.act[(size_t)k * a.B + idx], om = a.old_mean[(size_t)k * a.B + idx];
-        const double dm = om - mu;
-        if (a.loss_kind == B200RL_LOSS_KL) {
-          const double num = dm * dm + var_old[k] - var_new[k];
-          dmu[k] = -2.0 * dm / var_new2[k];
-          dls[k] = 1.0 - 2.0 * var_new[k] * (var_new2[k] + 2.0 * num) / (var_new2[k] * var_new2[k]);
-        } else {
-          double zsq = 0.0, zsq_old = 0.0;
-          for (int q = 0; q < A; ++q) {
-            double m2 = sp[N_::obo + q];
-            for (int j = 0; j < H; ++j) m2 = fma(ht[j], sp[N_::oWo + j * A + q], m2);
-            const double aq = a.act[(size_t)q * a.B + idx], oq = a.old_mean[(size_t)q * a.B + idx];
-            zsq += (aq - m2) * (aq - m2) / var_new[q];
-            zsq_old += (aq - oq) * (aq - oq) / var_old[q];
+      if constexpr (N_::CAT) {   // logit deltas: the term (or KL) gradient, or M J x from the forward sweep
+        for (int k = 0; k < A; ++k) dmu[k] = 0.0;
+        if (valid && MODE == MODE_FVP) {
+          for (int k = 0; k < A; ++k) dmu[k] = a.h64[(size_t)(H + k) * a.B + idx];
+        } else if (valid) {
+          double p[A], term, kl;
+          gru_cat_d<N_>(a, sp, ht, idx, p, term, kl, dmu);
+        }
+      } else {
+        for (int k = 0; k < A; ++k) {
+          dmu[k] = 0.0;
+          dls[k] = 0.0;
+          if (!valid) continue;
+          if (MODE == MODE_FVP) { dmu[k] = a.h64[(size_t)(H + k) * a.B + idx]; continue; }
+          double mu = sp[N_::obo + k];
+          for (int j = 0; j < H; ++j) mu = fma(ht[j], sp[N_::oWo + j * A + k], mu);
+          const double act = a.act[(size_t)k * a.B + idx], om = a.old_mean[(size_t)k * a.B + idx];
+          const double dm = om - mu;
+          if (a.loss_kind == B200RL_LOSS_KL) {
+            const double num = dm * dm + var_old[k] - var_new[k];
+            dmu[k] = -2.0 * dm / var_new2[k];
+            dls[k] = 1.0 - 2.0 * var_new[k] * (var_new2[k] + 2.0 * num) / (var_new2[k] * var_new2[k]);
+          } else {
+            double zsq = 0.0, zsq_old = 0.0;
+            for (int q = 0; q < A; ++q) {
+              double m2 = sp[N_::obo + q];
+              for (int j = 0; j < H; ++j) m2 = fma(ht[j], sp[N_::oWo + j * A + q], m2);
+              const double aq = a.act[(size_t)q * a.B + idx], oq = a.old_mean[(size_t)q * a.B + idx];
+              zsq += (aq - m2) * (aq - m2) / var_new[q];
+              zsq_old += (aq - oq) * (aq - oq) / var_old[q];
+            }
+            const double adv_s = a.adv[idx];
+            const double w_s = a.loss_kind == B200RL_LOSS_TRPO ? exp(-sum_ls_new - 0.5 * zsq + sum_ls_old + 0.5 * zsq_old) * adv_s
+                                                               : adv_s;
+            const double z = (act - mu) / exp(ls_new[k]);
+            dmu[k] = -w_s * z / exp(ls_new[k]);
+            dls[k] = -w_s * (z * z - 1.0);
           }
-          const double adv_s = a.adv[idx];
-          const double w_s = a.loss_kind == B200RL_LOSS_TRPO ? exp(-sum_ls_new - 0.5 * zsq + sum_ls_old + 0.5 * zsq_old) * adv_s
-                                                             : adv_s;
-          const double z = (act - mu) / exp(ls_new[k]);
-          dmu[k] = -w_s * z / exp(ls_new[k]);
-          dls[k] = -w_s * (z * z - 1.0);
         }
       }
       for (int k = 0; k < A; ++k) {
         atomicAdd(&acc[N_::obo + k], dmu[k]);
-        atomicAdd(&acc[N_::ols + k], dls[k]);
+        if constexpr (!N_::CAT) atomicAdd(&acc[N_::ols + k], dls[k]);
         for (int j = 0; j < H; ++j) atomicAdd(&acc[N_::oWo + j * A + k], ht[j] * dmu[k]);
       }
       double dprev[H];
@@ -1022,6 +1253,152 @@ int b200rl_gru_update_f64(int mode, int loss_kind, const double* params_f64, int
   const int A = (mode == MODE_GRAD && loss_kind == B200RL_LOSS_KL) ? 0 : act_dim;
   return launch_finalize_update(fin_f64(mode, ws, grid, P, vec_out, loss_out, scale, count,
                                         {ols, A, nullptr, params_f64, -INFINITY}, x, reg_coeff, diag_scale),
+                                st);
+}
+}
+
+// ---------------------------------------------------------------------------------------------- CategoricalGRUPolicy
+extern "C" {
+
+long long b200rl_categorical_gru_num_params(int obs_dim, int hidden, int n_actions, int include_action) {
+  B200RL_REQUIRE_GRU_CAT_SHAPE(obs_dim, hidden, n_actions, "categorical_gru_num_params");
+  long long P = 0;
+  B200RL_DISPATCH_GRU_CAT(include_action, { P = NetG::P; });
+  return P;
+}
+
+int b200rl_categorical_gru_get_actions(const float* params_f32, int obs_dim, int hidden, int n_actions,
+                                       int include_action, const float* obs, const float* prev_action,
+                                       const float* h_in, long long n, const float* u, unsigned int seed,
+                                       unsigned int iter, int row, long long lane0, int* act_out, float* prob_out,
+                                       float* h_out, void* stream) {
+  B200RL_REQUIRE(params_f32 && obs && n > 0 && act_out && prob_out && h_out, "categorical_gru_get_actions: bad arguments");
+  B200RL_REQUIRE_GRU_CAT_SHAPE(obs_dim, hidden, n_actions, "categorical_gru_get_actions");
+  const unsigned grid = (unsigned)((n + 127) / 128);
+  B200RL_DISPATCH_GRU_CAT(include_action, {
+    gru_cat_get_actions_kernel<NetG><<<grid, 128, 0, (cudaStream_t)stream>>>(params_f32, obs, prev_action, h_in, n, u,
+                                                                             seed, iter, row, lane0, act_out, prob_out,
+                                                                             h_out);
+  });
+  B200RL_LAUNCH_CHECK("gru_cat_get_actions_kernel");
+  return 0;
+}
+
+int b200rl_rollout_categorical_gru(int env_kind, const float* params_f32, int hidden, int include_action, int N, int T,
+                                   int max_path_length, const float* u, const float* reset_raw, unsigned int seed,
+                                   unsigned int iter, long long lane0, float* obs, float* act, float* prob, float* rew,
+                                   unsigned char* flags, unsigned short* tstep, void* stream) {
+  const RolloutArgs a{params_f32, 0.f, N, T, max_path_length, u, reset_raw, seed, iter, lane0,
+                      obs, act, prob, rew, flags, tstep, nullptr};
+  if (int rc = check_rollout_args("rollout_categorical_gru", a, false)) return rc;
+  if (env_kind != B200RL_ENV_GYM_CARTPOLE) {
+    set_error("rollout_categorical_gru: env kind %d is not compiled in for the categorical GRU policy (only %d, "
+              "CartPole-v0)", env_kind, B200RL_ENV_GYM_CARTPOLE);
+    return B200RL_EUNSUPPORTED;
+  }
+  B200RL_REQUIRE_GRU_CAT_SHAPE(GymCartPoleEnvD::O, hidden, EnvNumActions<GymCartPoleEnvD>::value,
+                               "rollout_categorical_gru");
+  B200RL_DISPATCH_GRU_CAT(include_action, {
+    gru_cat_rollout_kernel<GymCartPoleEnvD, NetG><<<(N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(a);
+  });
+  B200RL_LAUNCH_CHECK("gru_cat_rollout_kernel");
+  return 0;
+}
+
+int b200rl_categorical_gru_loss_kl(int loss_kind, const float* params_f32, int obs_dim, int hidden, int n_actions,
+                                   int include_action, int N, int T, const float* obs, const float* act,
+                                   const unsigned short* tstep, const float* adv, const float* old_prob,
+                                   const unsigned char* flags, double scale, const double* count, double* out,
+                                   float* h_cache_out, double* ws, void* stream) {
+  B200RL_REQUIRE(params_f32 && obs && act && tstep && adv && old_prob && out && ws && N > 0 && T > 0,
+                 "categorical_gru_loss_kl: bad arguments");
+  if (int rc = check_loss_kind("categorical_gru_loss_kl", loss_kind)) return rc;
+  B200RL_REQUIRE_GRU_CAT_SHAPE(obs_dim, hidden, n_actions, "categorical_gru_loss_kl");
+  cudaStream_t st = (cudaStream_t)stream;
+  GruArgs a{};
+  gru_fill(a, params_f32, N, T, obs, act, tstep, adv, old_prob, nullptr, loss_kind, flags, ws);
+  a.hbuf = h_cache_out;
+  const int grid = partial_grid(4, (N + 127) / 128);
+  B200RL_DISPATCH_GRU_CAT(include_action, { gru_loss_kernel<NetG><<<grid, 128, 0, st>>>(a); });
+  B200RL_LAUNCH_CHECK("gru_loss_kernel");
+  return launch_finalize_update(fin_loss(ws, grid, out, scale, count), st);
+}
+
+int b200rl_categorical_gru_grad(int loss_kind, double penalty, const float* params_f32, int obs_dim, int hidden,
+                                int n_actions, int include_action, int N, int T, const float* obs, const float* act,
+                                const unsigned short* tstep, const float* adv, const float* old_prob,
+                                const unsigned char* flags, double scale, const double* count, double* g_out,
+                                double* loss_out, float* h_cache, double* ws, void* stream) {
+  B200RL_REQUIRE(params_f32 && obs && act && tstep && adv && old_prob && g_out && h_cache && ws && N > 0 && T > 0,
+                 "categorical_gru_grad: bad arguments");
+  if (int rc = check_loss_kind("categorical_gru_grad", loss_kind)) return rc;
+  B200RL_REQUIRE(penalty >= 0.0 && penalty <= 3.0e38, "categorical_gru_grad: penalty must be finite and >= 0");
+  B200RL_REQUIRE_GRU_CAT_SHAPE(obs_dim, hidden, n_actions, "categorical_gru_grad");
+  cudaStream_t st = (cudaStream_t)stream;
+  GruArgs a{};
+  gru_fill(a, params_f32, N, T, obs, act, tstep, adv, old_prob, nullptr, loss_kind, flags, ws);
+  a.hbuf = h_cache;
+  a.penalty = (float)penalty;
+  int grid = 0, P = 0;
+  B200RL_DISPATCH_GRU_CAT(include_action, {
+    P = NetG::P;
+    int rc = launch_gru_bptt<NetG, MODE_GRAD>(a, &grid, st);
+    if (rc) return rc;
+  });
+  // no log_std block (A = 0): the gradient's min_std mask touches no entry
+  return launch_finalize_update(fin_grad(ws, grid, P, g_out, loss_out, scale, count, {P, 0, nullptr, nullptr, 0.0}), st);
+}
+
+int b200rl_categorical_gru_fvp(const float* params_f32, int obs_dim, int hidden, int n_actions, int include_action,
+                               int N, int T, const float* obs, const float* act, const unsigned short* tstep,
+                               const unsigned char* flags, const double* x, double scale, const double* count,
+                               double reg_coeff, double diag_scale, double* Hx_out, float* h_cache, int h_valid,
+                               float* plane, double* ws, void* stream) {
+  B200RL_REQUIRE(params_f32 && obs && act && tstep && x && Hx_out && h_cache && plane && ws && N > 0 && T > 0,
+                 "categorical_gru_fvp: bad arguments");
+  B200RL_REQUIRE_GRU_CAT_SHAPE(obs_dim, hidden, n_actions, "categorical_gru_fvp");
+  cudaStream_t st = (cudaStream_t)stream;
+  GruArgs a{};
+  gru_fill(a, params_f32, N, T, obs, act, tstep, nullptr, nullptr, nullptr, B200RL_LOSS_TRPO, flags, ws);
+  a.xvec = x; a.hbuf = h_cache; a.h_valid = h_valid ? 1 : 0;
+  a.plane = plane;   // the caller's [n][T][N] plane: M J x per sample, sized by the batch
+  int grid = 0, P = 0;
+  B200RL_DISPATCH_GRU_CAT(include_action, {
+    P = NetG::P;
+    int rc = launch_gru_bptt<NetG, MODE_FVP>(a, &grid, st);
+    if (rc) return rc;
+  });
+  return launch_finalize_update(fin_fvp(ws, grid, P, Hx_out, scale, count, {P, 0, params_f32, nullptr, 0.0}, x, reg_coeff,
+                                        diag_scale),   // no log_std block
+                                st);
+}
+
+int b200rl_categorical_gru_update_f64(int mode, int loss_kind, const double* params_f64, int obs_dim, int hidden,
+                                      int n_actions, int include_action, int N, int T, const float* obs,
+                                      const float* act, const unsigned short* tstep, const float* adv,
+                                      const float* old_prob, const unsigned char* flags, const double* x, double scale,
+                                      const double* count, double reg_coeff, double diag_scale, double* vec_out,
+                                      double* loss_out, double* h64, double* ws, void* stream) {
+  B200RL_REQUIRE(params_f64 && obs && act && tstep && h64 && ws && N > 0 && T > 0,
+                 "categorical_gru_update_f64: bad arguments");
+  if (int rc = check_f64_args("categorical_gru_update_f64", mode, loss_kind, adv && old_prob, x, vec_out, loss_out))
+    return rc;
+  B200RL_REQUIRE_GRU_CAT_SHAPE(obs_dim, hidden, n_actions, "categorical_gru_update_f64");
+  cudaStream_t st = (cudaStream_t)stream;
+  GruArgs64 a{};
+  a.params = params_f64; a.xvec = x; a.h64 = h64; a.N = N; a.T = T; a.B = (long long)N * T;
+  a.obs = obs; a.act = act; a.adv = adv; a.old_mean = old_prob; a.old_log_std = nullptr; a.tstep = tstep;
+  a.loss_kind = loss_kind; a.flags = flags; a.partial = ws;
+  int grid = 0, P = 0;
+  B200RL_DISPATCH_GRU_CAT(include_action, {
+    P = NetG::P;
+    int rc = (mode == MODE_LOSS) ? launch_gru_f64<NetG, MODE_LOSS>(a, &grid, st)
+           : (mode == MODE_GRAD) ? launch_gru_f64<NetG, MODE_GRAD>(a, &grid, st)
+                                 : launch_gru_f64<NetG, MODE_FVP>(a, &grid, st);
+    if (rc) return rc;
+  });
+  return launch_finalize_update(fin_f64(mode, ws, grid, P, vec_out, loss_out, scale, count,
+                                        {P, 0, nullptr, params_f64, 0.0}, x, reg_coeff, diag_scale),
                                 st);
 }
 }

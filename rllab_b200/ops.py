@@ -115,7 +115,8 @@ class CategoricalDims(tuple):
 
 
 def is_categorical(dims):
-    return isinstance(dims, CategoricalDims)
+    """A softmax policy over discrete actions (CategoricalMLPPolicy or CategoricalGRUPolicy): one-hot act, prob in mean."""
+    return isinstance(dims, (CategoricalDims, CategoricalGRUDims))
 
 
 class GRUDims(tuple):
@@ -135,6 +136,18 @@ def is_gru(dims):
     return isinstance(dims, GRUDims)
 
 
+class CategoricalGRUDims(GRUDims):
+    """(O, H, n, include_action) of a CategoricalGRUPolicy.  A GRUDims, so every recurrent-only rule holds for it (the
+    batch's recurrent layout, the rejections of CEM and of sub-sampled Fisher products); inside each GRU branch below it
+    selects the categorical GRU kernels (b200rl_categorical_gru_*), with batch.mean holding the old probabilities and
+    batch.act the one-hot actions, as for CategoricalDims."""
+
+
+def _gru_entry(dims, name):
+    """b200rl_gru_<name> or, for the categorical head, b200rl_categorical_gru_<name>."""
+    return ("b200rl_categorical_gru_" if isinstance(dims, CategoricalGRUDims) else "b200rl_gru_") + name
+
+
 def _gru_hbuf(batch, H):
     """[H][T][N] float32 hidden states of the GRU passes: the batch's activation cache buffer."""
     return batch.hcache(H, 0)
@@ -149,11 +162,26 @@ def _gru_h64(batch, H, A):
     return h
 
 
+def _cat_gru_plane(batch, n):
+    """[n][T][N] float32 scratch of the categorical GRU Fisher pass, M J x per sample (allocated on first use)."""
+    pl = getattr(batch, "_cat_gru_plane", None)
+    if pl is None or pl.shape[0] != n:
+        pl = torch.empty((n, batch.T, batch.N), dtype=F32, device=batch.device)
+        batch._cat_gru_plane = pl
+    return pl
+
+
 def gru_rollout(dims, params32, batch, max_path_length, kind, eps=None, reset_raw=None, seed=0, it=0, lane0=0):
     """Fused rollout with the GRU policy (b200rl_rollout_gru): b200rl_rollout's planes, h and prev_action per lane."""
     O, H, A, inc = dims
     b = batch
     _chk(params32, F32, "params32"), _chk(eps, F32, "eps"), _chk(reset_raw, F32, "reset_raw")
+    if isinstance(dims, CategoricalGRUDims):          # eps: the injected action uniforms u [T][N]
+        _chk(eps, F32, "u", b.T * b.N)
+        L.call("b200rl_rollout_categorical_gru", kind, L.ptr(params32), H, inc, b.N, b.T, max_path_length, L.ptr(eps),
+               L.ptr(reset_raw), seed, it, lane0, L.ptr(b.obs), L.ptr(b.act), L.ptr(b.mean), L.ptr(b.rew),
+               L.ptr(b.flags), L.ptr(b.tstep), _stream())
+        return
     L.call("b200rl_rollout_gru", kind, L.ptr(params32), H, inc, b.N, b.T, max_path_length, L.ptr(eps), L.ptr(reset_raw),
            seed, it, lane0, L.ptr(b.obs), L.ptr(b.act), L.ptr(b.mean), L.ptr(b.rew), L.ptr(b.flags), L.ptr(b.tstep),
            L.ptr(b.log_std), _stream())
@@ -169,6 +197,18 @@ def gru_get_actions(params32, dims, obs, prev_action, h_in, n, eps, seed, it, ro
     L.call("b200rl_gru_get_actions", L.ptr(params32), O, H, A, inc, L.ptr(obs), L.ptr(prev_action), L.ptr(h_in), n,
            L.ptr(eps), seed, it, row, lane0, L.ptr(act_out), L.ptr(mean_out), L.ptr(h_out), L.ptr(log_std_out),
            _stream())
+
+
+def categorical_gru_get_actions(params32, dims, obs, prev_action, h_in, n, u, seed, it, row, lane0, act_out, prob_out,
+                                h_out):
+    """One categorical GRU step of n rows (b200rl_categorical_gru_get_actions): act_out [n] int32, prob_out [n][n_rows],
+    h_out [H][n]; prev_action (one-hot) / h_in / u None = zeros / zeros / Philox."""
+    O, H, A, inc = dims
+    _chk(params32, F32, "params32"), _chk(obs, F32, "obs", O * n), _chk(prev_action, F32, "prev_action", A * n)
+    _chk(h_in, F32, "h_in", H * n), _chk(u, F32, "u", n), _chk(act_out, torch.int32, "act_out", n)
+    _chk(prob_out, F32, "prob_out", A * n), _chk(h_out, F32, "h_out", H * n)
+    L.call("b200rl_categorical_gru_get_actions", L.ptr(params32), O, H, A, inc, L.ptr(obs), L.ptr(prev_action),
+           L.ptr(h_in), n, L.ptr(u), seed, it, row, lane0, L.ptr(act_out), L.ptr(prob_out), L.ptr(h_out), _stream())
 
 
 _n_actions = {}
@@ -348,9 +388,10 @@ def loss_kl(loss_kind, params32, dims, min_std, batch, out, fuse=False):
     _chk(params32, F32, "params32"), _chk(out, F64, "out", 3)
     if is_gru(dims):
         O, H, A, inc = dims
+        head = (L.ptr(b.mean),) if is_categorical(dims) else (L.ptr(b.mean), L.ptr(b.log_std))
         with _Fused(fuse):
-            L.call("b200rl_gru_loss_kl", loss_kind, L.ptr(params32), O, H, A, inc, b.N, b.T, L.ptr(b.obs), L.ptr(b.act),
-                   L.ptr(b.tstep), L.ptr(b.adv), L.ptr(b.mean), L.ptr(b.log_std), fl, scale, cnt, L.ptr(out), None,
+            L.call(_gru_entry(dims, "loss_kl"), loss_kind, L.ptr(params32), O, H, A, inc, b.N, b.T, L.ptr(b.obs),
+                   L.ptr(b.act), L.ptr(b.tstep), L.ptr(b.adv), *head, fl, scale, cnt, L.ptr(out), None,
                    L.ptr(workspace(b.device)), _stream())
         return
     if is_categorical(dims):
@@ -418,9 +459,10 @@ def _gru_grad(loss_kind, penalty, params32, dims, batch, g_out, loss_out, h_cach
     fl, scale, cnt = _mask(b)
     hb = h_cache if h_cache is not None else _gru_hbuf(b, H)
     _chk(hb, F32, "h_cache", H * b.B)
+    head = (L.ptr(b.mean),) if is_categorical(dims) else (L.ptr(b.mean), L.ptr(b.log_std))
     with _Fused(fuse):
-        L.call("b200rl_gru_grad", loss_kind, float(penalty), L.ptr(params32), O, H, A, inc, b.N, b.T, L.ptr(b.obs),
-               L.ptr(b.act), L.ptr(b.tstep), L.ptr(b.adv), L.ptr(b.mean), L.ptr(b.log_std), fl, scale, cnt, L.ptr(g_out),
+        L.call(_gru_entry(dims, "grad"), loss_kind, float(penalty), L.ptr(params32), O, H, A, inc, b.N, b.T,
+               L.ptr(b.obs), L.ptr(b.act), L.ptr(b.tstep), L.ptr(b.adv), *head, fl, scale, cnt, L.ptr(g_out),
                L.ptr(loss_out), L.ptr(hb), L.ptr(workspace(b.device)), _stream())
 
 
@@ -441,10 +483,12 @@ def fvp(params32, dims, min_std, batch, x, reg_coeff, diag_scale, Hx_out, h_cach
         O, H, A, inc = dims
         hb = h_cache if h_cache is not None else _gru_hbuf(b, H)
         _chk(hb, F32, "h_cache", H * b.B)
+        # the categorical head's M J x plane is sized by the batch; the Gaussian one lives in the workspace
+        plane = (L.ptr(_cat_gru_plane(b, A)),) if is_categorical(dims) else ()
         with _Fused(fuse):
-            L.call("b200rl_gru_fvp", L.ptr(params32), O, H, A, inc, b.N, b.T, L.ptr(b.obs), L.ptr(b.act), L.ptr(b.tstep),
+            L.call(_gru_entry(dims, "fvp"), L.ptr(params32), O, H, A, inc, b.N, b.T, L.ptr(b.obs), L.ptr(b.act), L.ptr(b.tstep),
                    fl, L.ptr(x), scale, cnt, float(reg_coeff), float(diag_scale), L.ptr(Hx_out), L.ptr(hb),
-                   int(h_cache is not None), L.ptr(workspace(b.device)), _stream())
+                   int(h_cache is not None), *plane, L.ptr(workspace(b.device)), _stream())
         return
     if is_categorical(dims):
         with _Fused(fuse):
@@ -472,9 +516,10 @@ def update_f64(mode, loss_kind, params64, dims, min_std, batch, x, reg_coeff, di
     _chk(params64, F64, "params64"), _chk(x, F64, "x"), _chk(vec_out, F64, "vec_out"), _chk(loss_out, F64, "loss_out", 3)
     if is_gru(dims):
         O, H, A, inc = dims
+        head = (L.ptr(b.mean),) if is_categorical(dims) else (L.ptr(b.mean), L.ptr(b.log_std))
         with _Fused(fuse):
-            L.call("b200rl_gru_update_f64", mode, loss_kind, L.ptr(params64), O, H, A, inc, b.N, b.T, L.ptr(b.obs),
-                   L.ptr(b.act), L.ptr(b.tstep), L.ptr(b.adv), L.ptr(b.mean), L.ptr(b.log_std), fl, L.ptr(x), scale, cnt,
+            L.call(_gru_entry(dims, "update_f64"), mode, loss_kind, L.ptr(params64), O, H, A, inc, b.N, b.T,
+                   L.ptr(b.obs), L.ptr(b.act), L.ptr(b.tstep), L.ptr(b.adv), *head, fl, L.ptr(x), scale, cnt,
                    float(reg_coeff), float(diag_scale), L.ptr(vec_out), L.ptr(loss_out), L.ptr(_gru_h64(b, H, A)),
                    L.ptr(workspace(b.device)), _stream())
         return
