@@ -576,6 +576,98 @@ int b200rl_reps_dual_sums(int obs_dim, int N, int T, const float* obs, const flo
  * (samples_data["observations"] etc., rllab/sampler/base.py:74-104): dst[(t*N+n)*dim + k] = src[k][t][n]. */
 int b200rl_planes_to_rows_f64(int dim, long long B, const float* src, double* dst, void* stream);
 
+/* ---- DDPG (rllab/algos/ddpg.py) with DeterministicMLPPolicy and ContinuousMLPQFunction. ----
+ * Env kinds: the classic-control Box kinds (point, cartpole, pendulum, cartpole_swingup, double_pendulum); planar and
+ * discrete kinds return B200RL_EUNSUPPORTED.  Both nets are (32, 32) with ReLU hidden units.
+ *   policy (deterministic_mlp_policy.py): [h0.W (O,32), h0.b, h1.W (32,32), h1.b, output.W (32,A), output.b], tanh out;
+ *   qf (continuous_mlp_q_function.py, action_merge_layer = -2): [h1.W (O,32), h1.b, h2.W (32+A,32) (hidden rows, then
+ *   action rows), h2.b, output.W (32,1), output.b], linear out.
+ * A run's network state `nets` is [4][P] float64 with P = P_policy + P_qf: theta, Adam m, Adam v, target, each laid out
+ * [policy | qf].  Adam is lasagne.updates.adam (beta1 0.9, beta2 0.999, epsilon 1e-8) with one step count for both
+ * nets.  Minibatch size 32.
+ *
+ * Philox draws of run r at step itr (itr_lo = itr & 0x0FFFFFFF, itr_hi = itr >> 28):
+ *   counter (r, itr_lo | stream << 28, sub, 0), key (seed, itr_hi)
+ *   stream 1 (the reset stream): sub = chunk; a path's reset at step itr (the first reset at itr = 0)
+ *   stream B200RL_DDPG_STREAM_EXPLORE: sub = chunk c holds the N(0,1) draws of action entries 4c..4c+3 (Box-Muller on
+ *     word pairs, u = (w + 0.5) * 2^-32, float64: rad = sqrt(-2 log u0), n0 = rad cos(2 pi u1), n1 = rad sin(2 pi u1))
+ *   stream B200RL_DDPG_STREAM_INDEX: sub = (update << 16) | (candidate >> 2), word candidate & 3; candidate j of update
+ *     `update` maps to index = (bottom + ((uint64)w * size >> 32)) % replay_pool_size and is rejected when
+ *     index == size - 1 (SimpleReplayPool.random_batch); the first 32 accepted candidates form the minibatch. */
+#define B200RL_DDPG_BATCH 32
+#define B200RL_DDPG_STREAM_EXPLORE 3
+#define B200RL_DDPG_STREAM_INDEX 4
+#define B200RL_ES_OU 0       /* rllab/exploration_strategies/ou_strategy.py */
+#define B200RL_ES_GAUSSIAN 1 /* rllab/exploration_strategies/gaussian_strategy.py */
+/* per-run statistics, float64, summed over the updates of every launch since the caller last cleared them */
+#define B200RL_DDPG_NSTAT 9  /* n_updates, qf_loss, policy_surr, q, |q|, y, |y|, |q - y|, n_es_returns */
+
+typedef struct {
+  int n_updates_per_sample, max_path_length, min_pool_size, replay_pool_size;
+  int include_horizon_terminal_transitions, es_kind;
+  double discount, scale_reward, soft_target_tau;
+  double qf_weight_decay, qf_learning_rate, policy_weight_decay, policy_learning_rate;
+  double ou_mu, ou_theta, ou_sigma;                   /* OUStrategy */
+  double gs_max_sigma, gs_min_sigma, gs_decay_period; /* GaussianStrategy */
+} b200rl_ddpg_hparams;
+
+/* The train() loop's state of one run between launches.  terminal: 0 = inside a path, 1 = the last step ended a path
+ * (the next step resets and records path_return as an Es return), 2 = a fresh run (the next step resets, no return). */
+typedef struct {
+  float env_state[8];
+  float obs[8];
+  double ou_state[4];
+  double path_return;
+  long long itr, adam_t;
+  int path_length, terminal, top, bottom, size, pad_;
+} b200rl_ddpg_state;
+
+typedef struct {
+  int env_kind, f64;      /* f64: nets, backward passes and Adam in float64 (parity mode); the env is float32 always */
+  int n_runs, n_steps;    /* one CTA per run; n_steps of the train() loop per launch */
+  int es_cap;             /* capacity of each run's es_returns row */
+  unsigned int seed;
+  b200rl_ddpg_hparams hp;
+  b200rl_ddpg_state* state;   /* [n_runs] */
+  double* nets;               /* [n_runs][4][P] */
+  float* pool_obs;            /* [n_runs][replay_pool_size][O] */
+  float* pool_act;            /* [n_runs][replay_pool_size][A] */
+  float* pool_rew;            /* [n_runs][replay_pool_size], reward * scale_reward */
+  unsigned char* pool_term;   /* [n_runs][replay_pool_size] */
+  double* stats;              /* [n_runs][B200RL_DDPG_NSTAT], accumulated */
+  double* es_returns;         /* [n_runs][es_cap]: returns of the finished exploration paths, at stats[8] */
+  void* stream;
+} b200rl_ddpg_train_args;
+
+/* P of the policy (which = 0) or the Q function (which = 1); negative when (obs_dim, act_dim) is not compiled in. */
+long long b200rl_ddpg_num_params(int obs_dim, int act_dim, int which);
+
+/* DeterministicMLPPolicy.get_actions: obs [O][n], act_out [A][n], policy parameters float32. */
+int b200rl_deterministic_get_actions(const float* params_f32, int obs_dim, int act_dim, const float* obs, long long n,
+                                     float* act_out, void* stream);
+
+/* ContinuousMLPQFunction.get_qval: obs [O][n], act [A][n], q_out [n], Q parameters float32. */
+int b200rl_qf_get_qval(const float* params_f32, int obs_dim, int act_dim, const float* obs, const float* act,
+                       long long n, float* q_out, void* stream);
+
+/* Noise-free lane rollout of the deterministic policy (the paths DDPG.evaluate samples), layouts of b200rl_rollout;
+ * act receives the policy's output. */
+int b200rl_rollout_deterministic(int env_kind, const float* params_f32, int N, int T, int max_path_length,
+                                 const float* reset_raw, unsigned int seed, unsigned int iter, long long lane0, float* obs,
+                                 float* act, float* rew, unsigned char* flags, unsigned short* tstep, void* stream);
+
+/* One DDPG.do_training on the minibatch idx [32] (int) of one run's pool (layouts of b200rl_ddpg_train_args, pool of
+ * pool_size rows): updates nets [4][P] in place with Adam step adam_t (>= 1) and writes grad_out [P] (the two loss
+ * gradients with their weight decay, [policy | qf]), qval_out [32] and y_out [32] (float64) and
+ * loss_out [2] = (qf_loss, policy_surr), both before their update.  Runs the fused loop's update code. */
+int b200rl_ddpg_update(int env_kind, int f64, const b200rl_ddpg_hparams* hp, const float* pool_obs,
+                       const float* pool_act, const float* pool_rew, const unsigned char* pool_term, int pool_size,
+                       const int* idx, double* nets, long long adam_t, double* grad_out, double* qval_out,
+                       double* y_out, double* loss_out, void* stream);
+
+/* n_steps of DDPG.train()'s loop for n_runs independent runs in one launch; see b200rl_ddpg_train_args. */
+int b200rl_ddpg_train(const b200rl_ddpg_train_args* args);
+
 #ifdef __cplusplus
 }
 #endif

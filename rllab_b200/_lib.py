@@ -28,6 +28,34 @@ PS_NSUM, PS_NMAX = 16, 4
 _P = c_void_p
 _LL = c_longlong
 
+DDPG_BATCH, DDPG_NSTAT = 32, 9
+DDPG_STREAM_EXPLORE, DDPG_STREAM_INDEX = 3, 4
+ES_OU, ES_GAUSSIAN = 0, 1
+
+
+class DdpgHparams(ctypes.Structure):
+    """b200rl_ddpg_hparams."""
+    _fields_ = [(n, c_int) for n in ("n_updates_per_sample", "max_path_length", "min_pool_size", "replay_pool_size",
+                                     "include_horizon_terminal_transitions", "es_kind")] + \
+               [(n, c_double) for n in ("discount", "scale_reward", "soft_target_tau", "qf_weight_decay",
+                                        "qf_learning_rate", "policy_weight_decay", "policy_learning_rate", "ou_mu",
+                                        "ou_theta", "ou_sigma", "gs_max_sigma", "gs_min_sigma", "gs_decay_period")]
+
+
+class DdpgState(ctypes.Structure):
+    """b200rl_ddpg_state: one run's train() loop state between launches."""
+    _fields_ = [("env_state", c_float * 8), ("obs", c_float * 8), ("ou_state", c_double * 4), ("path_return", c_double),
+                ("itr", c_longlong), ("adam_t", c_longlong), ("path_length", c_int), ("terminal", c_int),
+                ("top", c_int), ("bottom", c_int), ("size", c_int), ("pad_", c_int)]
+
+
+class DdpgTrainArgs(ctypes.Structure):
+    """b200rl_ddpg_train_args."""
+    _fields_ = [("env_kind", c_int), ("f64", c_int), ("n_runs", c_int), ("n_steps", c_int), ("es_cap", c_int),
+                ("seed", c_uint), ("hp", DdpgHparams), ("state", c_void_p), ("nets", c_void_p),
+                ("pool_obs", c_void_p), ("pool_act", c_void_p), ("pool_rew", c_void_p), ("pool_term", c_void_p),
+                ("stats", c_void_p), ("es_returns", c_void_p), ("stream", c_void_p)]
+
 # name -> (restype, argtypes).  Mirrors include/b200rl.h one to one (tests/test_abi.py checks the header against this).
 SIGNATURES = {
     "b200rl_last_error": (c_char_p, []),
@@ -134,6 +162,14 @@ SIGNATURES = {
                                            _P, c_double, c_double, _P, _P, c_int, _P, _P, _P]),
     "b200rl_categorical_gru_update_f64": (c_int, [c_int, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P,
                                                   _P, _P, _P, _P, c_double, _P, c_double, c_double, _P, _P, _P, _P, _P]),
+    "b200rl_ddpg_num_params": (_LL, [c_int, c_int, c_int]),
+    "b200rl_deterministic_get_actions": (c_int, [_P, c_int, c_int, _P, _LL, _P, _P]),
+    "b200rl_qf_get_qval": (c_int, [_P, c_int, c_int, _P, _P, _LL, _P, _P]),
+    "b200rl_rollout_deterministic": (c_int, [c_int, _P, c_int, c_int, c_int, _P, c_uint, c_uint, _LL, _P, _P, _P, _P,
+                                             _P, _P]),
+    "b200rl_ddpg_update": (c_int, [c_int, c_int, POINTER(DdpgHparams), _P, _P, _P, _P, c_int, _P, _P, _LL, _P, _P, _P,
+                                   _P, _P]),
+    "b200rl_ddpg_train": (c_int, [POINTER(DdpgTrainArgs)]),
 }
 
 _lib = None
@@ -239,3 +275,12 @@ def categorical_gru_num_params(O, H, n, include_action):
     if p < 0:
         raise B200RLError("unsupported categorical GRU network O=%d hidden=%d n=%d: %s" % (O, H, n, last_error()))
     return int(p)
+
+
+def ddpg_num_params(O, A):
+    """(P_policy, P_qf) of the DDPG nets at (obs_dim, act_dim)."""
+    lib = load()
+    pp, qp = lib.b200rl_ddpg_num_params(O, A, 0), lib.b200rl_ddpg_num_params(O, A, 1)
+    if pp < 0 or qp < 0:
+        raise B200RLError("unsupported DDPG networks O=%d A=%d: %s" % (O, A, last_error()))
+    return int(pp), int(qp)

@@ -707,3 +707,108 @@ class LazyTriple(object):
 
     def __iter__(self):
         return iter(self.values())
+
+
+# ---------------------------------------------------------------- DDPG (rllab_b200/csrc/ddpg.cu)
+def deterministic_get_actions(params32, O, A, obs, n, act_out):
+    """DeterministicMLPPolicy forward: obs [O][n] -> act_out [A][n]."""
+    _chk(params32, F32, "params32"), _chk(obs, F32, "obs", O * n), _chk(act_out, F32, "act_out", A * n)
+    L.call("b200rl_deterministic_get_actions", L.ptr(params32), O, A, L.ptr(obs), n, L.ptr(act_out), _stream())
+
+
+def qf_get_qval(params32, O, A, obs, act, n, q_out):
+    """ContinuousMLPQFunction forward: obs [O][n], act [A][n] -> q_out [n]."""
+    _chk(params32, F32, "params32"), _chk(obs, F32, "obs", O * n), _chk(act, F32, "act", A * n)
+    _chk(q_out, F32, "q_out", n)
+    L.call("b200rl_qf_get_qval", L.ptr(params32), O, A, L.ptr(obs), L.ptr(act), n, L.ptr(q_out), _stream())
+
+
+def rollout_deterministic(kind, params32, batch, max_path_length, reset_raw=None, seed=0, it=0, lane0=0):
+    """Noise-free rollout of the deterministic policy into a LaneBatch (batch.mean is left untouched)."""
+    b = batch
+    _chk(params32, F32, "params32"), _chk(reset_raw, F32, "reset_raw")
+    L.call("b200rl_rollout_deterministic", kind, L.ptr(params32), b.N, b.T, max_path_length, L.ptr(reset_raw), seed,
+           it, lane0, L.ptr(b.obs), L.ptr(b.act), L.ptr(b.rew), L.ptr(b.flags), L.ptr(b.tstep), _stream())
+
+
+def ddpg_hparams(**kw):
+    """b200rl_ddpg_hparams from keyword arguments (every field required)."""
+    hp = L.DdpgHparams()
+    for name, _ in L.DdpgHparams._fields_:
+        setattr(hp, name, kw[name])
+    return hp
+
+
+def ddpg_update(kind, f64, hp, pool_obs, pool_act, pool_rew, pool_term, idx, nets, adam_t, grad_out, qval_out, y_out,
+                loss_out):
+    """One DDPG.do_training on one run's pool (b200rl_ddpg_update); nets [4][P] float64 is updated in place."""
+    rows = pool_rew.numel()
+    _chk(pool_obs, F32, "pool_obs"), _chk(pool_act, F32, "pool_act"), _chk(pool_rew, F32, "pool_rew")
+    _chk(pool_term, U8, "pool_term", rows), _chk(idx, torch.int32, "idx", L.DDPG_BATCH), _chk(nets, F64, "nets")
+    _chk(grad_out, F64, "grad_out", nets.numel() // 4), _chk(qval_out, F64, "qval_out", L.DDPG_BATCH)
+    _chk(y_out, F64, "y_out", L.DDPG_BATCH), _chk(loss_out, F64, "loss_out", 2)
+    L.call("b200rl_ddpg_update", kind, int(bool(f64)), ctypes.byref(hp), L.ptr(pool_obs), L.ptr(pool_act),
+           L.ptr(pool_rew), L.ptr(pool_term), rows, L.ptr(idx), L.ptr(nets), int(adam_t), L.ptr(grad_out),
+           L.ptr(qval_out), L.ptr(y_out), L.ptr(loss_out), _stream())
+
+
+class DdpgRuns(object):
+    """Device state of n_runs independent DDPG runs (b200rl_ddpg_train_args): loop state, nets [n_runs][4][P], replay
+    pools and statistics.  train(n_steps) advances every run by n_steps of DDPG.train()'s loop in one launch."""
+
+    def __init__(self, kind, O, A, n_runs, hp, nets64, seed, device, f64=False, es_cap=None):
+        self.kind, self.O, self.A, self.n_runs, self.hp, self.seed, self.f64 = kind, O, A, n_runs, hp, seed, f64
+        self.device = device
+        rows = hp.replay_pool_size
+        self.nets = torch.as_tensor(np.asarray(nets64, np.float64)).reshape(n_runs, 4, -1).to(device).contiguous()
+        self.P = self.nets.shape[2]
+        st = (L.DdpgState * n_runs)()
+        for r in range(n_runs):
+            st[r].terminal = 2
+        self.state = torch.frombuffer(bytearray(bytes(st)), dtype=U8).to(device)
+        self.pool_obs = torch.zeros((n_runs, rows, O), dtype=F32, device=device)
+        self.pool_act = torch.zeros((n_runs, rows, A), dtype=F32, device=device)
+        self.pool_rew = torch.zeros((n_runs, rows), dtype=F32, device=device)
+        self.pool_term = torch.zeros((n_runs, rows), dtype=U8, device=device)
+        self.stats = torch.zeros((n_runs, L.DDPG_NSTAT), dtype=F64, device=device)
+        self.es_cap = int(es_cap or 1)
+        self.es_returns = torch.zeros((n_runs, self.es_cap), dtype=F64, device=device)
+
+    def train(self, n_steps):
+        """n_steps loop iterations of every run in one launch.  A path ends at most once per step, so the Es return buffer
+        is grown to one entry per step since the last take_stats (no device readback needed)."""
+        self._pending = getattr(self, "_pending", 0) + int(n_steps)   # steps since the last take_stats
+        need = self._pending + 1
+        if need > self.es_cap:
+            grown = torch.zeros((self.n_runs, need), dtype=F64, device=self.device)
+            grown[:, :self.es_cap] = self.es_returns
+            self.es_returns, self.es_cap = grown, need
+        a = L.DdpgTrainArgs(env_kind=self.kind, f64=int(bool(self.f64)), n_runs=self.n_runs, n_steps=int(n_steps),
+                            es_cap=self.es_cap, seed=self.seed, hp=self.hp, state=self.state.data_ptr(),
+                            nets=self.nets.data_ptr(), pool_obs=self.pool_obs.data_ptr(),
+                            pool_act=self.pool_act.data_ptr(), pool_rew=self.pool_rew.data_ptr(),
+                            pool_term=self.pool_term.data_ptr(), stats=self.stats.data_ptr(),
+                            es_returns=self.es_returns.data_ptr(),
+                            stream=torch.cuda.current_stream().cuda_stream)
+        L.call("b200rl_ddpg_train", ctypes.byref(a))
+
+    def host_state(self):
+        """The runs' b200rl_ddpg_state structs, copied to the host."""
+        raw = bytes(self.state.cpu().numpy().tobytes())
+        return list((L.DdpgState * self.n_runs).from_buffer_copy(raw))
+
+    def set_host_state(self, states):
+        arr = (L.DdpgState * self.n_runs)(*states)
+        self.state.copy_(torch.frombuffer(bytearray(bytes(arr)), dtype=U8))
+
+    def take_stats(self):
+        """(stats [n_runs][NSTAT], list of Es-return arrays) accumulated since the last call, then cleared."""
+        stats = self.stats.cpu().numpy().copy()
+        es = self.es_returns.cpu().numpy()
+        n = stats[:, 8].astype(np.int64)
+        if (n > self.es_cap).any():
+            raise RuntimeError("ddpg: Es return buffer overflow (%d > %d)" % (n.max(), self.es_cap))
+        out = [es[r, :n[r]].copy() for r in range(self.n_runs)]
+        self.stats.zero_()
+        self._pending = 0
+        return stats, out
