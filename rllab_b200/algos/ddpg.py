@@ -70,6 +70,8 @@ class DDPG(RLAlgorithm):
     def hparams(self):
         from .. import ops
         es = self.es
+        # only the chosen strategy's parameters: GaussianStrategy.sigma is a method, not OUStrategy's sigma
+        ou = es.ES_KIND == L.ES_OU
         return ops.ddpg_hparams(
             n_updates_per_sample=self.n_updates_per_sample, max_path_length=self.max_path_length,
             min_pool_size=self.min_pool_size, replay_pool_size=self.replay_pool_size,
@@ -77,10 +79,10 @@ class DDPG(RLAlgorithm):
             es_kind=es.ES_KIND, discount=self.discount, scale_reward=self.scale_reward,
             soft_target_tau=self.soft_target_tau, qf_weight_decay=self.qf_weight_decay,
             qf_learning_rate=self.qf_learning_rate, policy_weight_decay=self.policy_weight_decay,
-            policy_learning_rate=self.policy_learning_rate, ou_mu=getattr(es, "mu", 0.0),
-            ou_theta=getattr(es, "theta", 0.0), ou_sigma=getattr(es, "sigma", 0.0),
-            gs_max_sigma=getattr(es, "_max_sigma", 0.0), gs_min_sigma=getattr(es, "_min_sigma", 0.0),
-            gs_decay_period=getattr(es, "_decay_period", 1.0))
+            policy_learning_rate=self.policy_learning_rate, ou_mu=es.mu if ou else 0.0,
+            ou_theta=es.theta if ou else 0.0, ou_sigma=es.sigma if ou else 0.0,
+            gs_max_sigma=0.0 if ou else es._max_sigma, gs_min_sigma=0.0 if ou else es._min_sigma,
+            gs_decay_period=1.0 if ou else es._decay_period)
 
     def init_opt(self):
         import copy

@@ -221,11 +221,13 @@ def gather(pool, idx, rows):
                 s2=pool["obs"][(idx + 1) % rows].astype(np.float64))
 
 
-def train_step(d, st, hp, seed, run, env_reset, env_step, stats=None, record=None):
+def train_step(d, st, hp, seed, run, env_reset, env_step, stats=None, record=None, action=None, explored=None):
     """One iteration of DDPG.train()'s loop on the run state st (modified in place).  env_reset(itr) -> (env_state, obs)
     and env_step(env_state, action float32 in [-1, 1]) -> (env_state, obs, reward, done) are the env.  stats: optional
     dict of lists (es_returns, qf_loss, policy_surr, q, y); record: optional list that receives each update's
-    (indices, info, rejected indices)."""
+    (indices, info, rejected indices), info["grad"] being the update's gradient.  action: optional float32 [A] that is
+    stepped and stored in the pool instead of the oracle's own clipped action (the exploration state still advances);
+    explored: optional list that receives the oracle's own clip(mu + noise, -1, 1) in float64."""
     rows = hp["replay_pool_size"]
     if st["terminal"]:
         st["env_state"], st["obs"] = env_reset(st["itr"])
@@ -240,7 +242,9 @@ def train_step(d, st, hp, seed, run, env_reset, env_step, stats=None, record=Non
         x = mu[0] + st["ou"]
     else:
         x = mu[0] + nz * gaussian_sigma(st["itr"], hp["gs_max_sigma"], hp["gs_min_sigma"], hp["gs_decay_period"])
-    act = np.clip(x, -1.0, 1.0).astype(np.float32)
+    if explored is not None:
+        explored.append(np.clip(x, -1.0, 1.0))
+    act = np.clip(x, -1.0, 1.0).astype(np.float32) if action is None else np.asarray(action, np.float32)
     env_state, obs2, r, done = env_step(st["env_state"], act)
     st["path_length"] += 1
     st["path_return"] += float(r)
