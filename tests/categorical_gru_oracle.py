@@ -51,16 +51,20 @@ def _flat_batch(lanes, p):
                 adv=lanes["adv"].astype(np.float64).reshape(-1))
 
 
-def terms(flat, lanes, dims, kind):
-    """Per-sample surrogate term and KL (T, N)."""
-    p, _, _ = forward(flat, lanes, dims)
-    fb = _flat_batch(lanes, p)
-    pf = p.reshape(-1, dims.A)
+def _terms(p, fb, kind):
+    """Per-sample surrogate term and KL (T, N) of the probabilities p (T, N, n) over the sample dict fb."""
+    pf = p.reshape(-1, p.shape[-1])
     if kind == "trpo":
         term = -CO.likelihood_ratio(fb["actions"], fb["old_prob"], pf) * fb["adv"]
     else:
         term = -CO.log_likelihood(fb["actions"], pf) * fb["adv"]
     return term.reshape(p.shape[:2]), CO.kl(fb["old_prob"], pf).reshape(p.shape[:2])
+
+
+def terms(flat, lanes, dims, kind):
+    """Per-sample surrogate term and KL (T, N)."""
+    p, _, _ = forward(flat, lanes, dims)
+    return _terms(p, _flat_batch(lanes, p), kind)
 
 
 def loss_kl(flat, lanes, dims, kind):
@@ -82,6 +86,40 @@ def grad(flat, lanes, dims, kind, penalty=0.0):
     v = GO.valid_of(lanes)
     dz = np.where(v[..., None], dz.reshape(p.shape), 0.0) / v.sum()
     return GO._bptt(flat, dims, cache, dz, np.zeros_like(dz))
+
+
+def log_ratio(flat, lanes, dims):
+    """Per-sample log p[a] - log q[a] of the taken action (with TINY, as the likelihood terms), (T, N)."""
+    p, _, _ = forward(flat, lanes, dims)
+    fb = _flat_batch(lanes, p)
+    lr = CO.log_likelihood(fb["actions"], p.reshape(-1, dims.A)) - CO.log_likelihood(fb["actions"], fb["old_prob"])
+    return lr.reshape(p.shape[:2])
+
+
+def lbfgs_step(optimizer, theta0, lanes, dims, kind, step_size=None):
+    """gru_oracle.lbfgs_step over this policy's loss / KL and gradient: PPO (PenaltyLbfgsOptimizer) or ERWR
+    (LbfgsOptimizer) from theta0 with float64 callables."""
+    return GO.lbfgs_step(optimizer, theta0, lanes, dims, kind, step_size, loss_kl=loss_kl, grad=grad)
+
+
+def pass_refs(flat, lanes, dims):
+    """What the update passes compute at flat, from one forward sweep: {kind: (surrogate, mean KL, max KL)} and
+    {kind: gradient} for kinds "trpo" and "vpg", and the gradient of mean KL under "kl" (gru_oracle.pass_refs)."""
+    p, _, cache = forward(flat, lanes, dims)
+    fb = _flat_batch(lanes, p)
+    pf = p.reshape(-1, dims.A)
+    v = GO.valid_of(lanes)
+    tri, g = {}, {}
+    for kind in ("trpo", "vpg", "kl"):
+        if kind == "kl":
+            dz = CO._kl_logit_grad(pf, fb["old_prob"])
+        else:
+            term, kl = _terms(p, fb, kind)
+            tri[kind] = (term[v].mean(), kl[v].mean(), kl[v].max())
+            dz = CO.logit_grad(pf, fb, kind)
+        dz = np.where(v[..., None], dz.reshape(p.shape), 0.0) / v.sum()
+        g[kind] = GO._bptt(flat, dims, cache, dz, np.zeros_like(dz))
+    return tri, g
 
 
 def fvp(flat, lanes, dims, xvec, reg_coeff=1e-5):

@@ -5,7 +5,7 @@ linear mean head, the recurrent dist_info_sym of rllab/policies/gaussian_gru_pol
 and the NPO / VPG surrogates and mean / max KL with valids (npo.py:67-82, vpg.py:66-90) over it.  Lanes are time-major
 planes [dim][T][N] with tstep; a path starts where tstep == 0: h = 0 and prev_action = 0 there, otherwise prev_action is
 act[t-1] of the lane.  Gradients by backpropagation through time, the Fisher-vector product J^T M J x by a forward
-tangent sweep, and a TRPO step.  Flat layout [W_xr, W_hr, b_r, W_xu, W_hu, b_u, W_xc, W_hc, b_c, W_out, b_out, log_std].
+tangent sweep, a TRPO step, and the host L-BFGS optimizers (PPO, ERWR) driven by these float64 callables.  Flat layout [W_xr, W_hr, b_r, W_xu, W_hu, b_u, W_xc, W_hc, b_c, W_out, b_out, log_std].
 """
 import numpy as np
 
@@ -95,10 +95,11 @@ def valid_of(lanes):
     return lanes.get("valid", np.ones(lanes["tstep"].shape, dtype=bool))
 
 
-def _terms(flat, lanes, dims, kind, penalty=0.0):
-    """Per-sample (term, kl, dmu, dls) (dmu, dls [T][N][A]) and the mean (A, T, N)."""
+def _terms(flat, lanes, dims, kind, penalty=0.0, fwd=None):
+    """Per-sample (term, kl, dmu, dls) (dmu, dls [T][N][A]) and the forward cache; fwd: forward()'s result at flat,
+    if already computed."""
     p = unpack(flat, dims)
-    mean, cache = forward(flat, lanes, dims)
+    mean, cache = forward(flat, lanes, dims) if fwd is None else fwd
     ls, ls_old = p["log_std"], np.asarray(lanes["old_log_std"], dtype=np.float64)
     mu = np.moveaxis(mean, 0, -1)
     act = np.moveaxis(lanes["act"].astype(np.float64), 0, -1)
@@ -138,6 +139,16 @@ def loss_kl(flat, lanes, dims, kind):
     return term[v].mean(), kl[v].mean(), kl[v].max()
 
 
+def log_ratio(flat, lanes, dims):
+    """Per-sample log likelihood ratio log pi_theta(a) - log pi_old(a) of the recorded actions, [T][N]."""
+    mu = np.moveaxis(forward(flat, lanes, dims)[0], 0, -1)
+    ls, ls_old = unpack(flat, dims)["log_std"], np.asarray(lanes["old_log_std"], dtype=np.float64)
+    act = np.moveaxis(lanes["act"].astype(np.float64), 0, -1)
+    om = np.moveaxis(lanes["old_mean"].astype(np.float64), 0, -1)
+    z, zo = (act - mu) / np.exp(ls), (act - om) / np.exp(ls_old)
+    return ls_old.sum() - ls.sum() - 0.5 * np.sum(z * z - zo * zo, -1)
+
+
 def _bptt(flat, dims, cache, dmu, dls):
     """Flat gradient from per-sample output deltas dmu [T][N][A] (already masked and scaled) and dls [T][N][A]."""
     p = unpack(flat, dims)
@@ -163,14 +174,74 @@ def _bptt(flat, dims, cache, dmu, dls):
     return pack(g, dims)
 
 
+def _valid_bptt(flat, lanes, dims, cache, dmu, dls):
+    """_bptt of the per-sample deltas averaged over the valid samples."""
+    v = valid_of(lanes)
+    n = v.sum()
+    return _bptt(flat, dims, cache, np.where(v[..., None], dmu, 0.0) / n, np.where(v[..., None], dls, 0.0) / n)
+
+
 def grad(flat, lanes, dims, kind, penalty=0.0):
     """Gradient of the surrogate (+ penalty * mean KL); kind "kl": gradient of mean KL."""
     _, _, dmu, dls, cache = _terms(flat, lanes, dims, kind, penalty)
+    return _valid_bptt(flat, lanes, dims, cache, dmu, dls)
+
+
+def pass_refs(flat, lanes, dims):
+    """What the update passes compute at flat, from one forward sweep: {kind: (surrogate, mean KL, max KL)} and
+    {kind: gradient} for kinds "trpo" and "vpg", and the gradient of mean KL under "kl".  The penalised gradient is
+    grad[kind] + penalty * grad["kl"] (the objective is linear in the penalty)."""
+    fwd = forward(flat, lanes, dims)
     v = valid_of(lanes)
-    n = v.sum()
-    dmu = np.where(v[..., None], dmu, 0.0) / n
-    dls = np.where(v[..., None], dls, 0.0) / n
-    return _bptt(flat, dims, cache, dmu, dls)
+    tri, g = {}, {}
+    for kind in ("trpo", "vpg", "kl"):
+        term, kl, dmu, dls, cache = _terms(flat, lanes, dims, kind, fwd=fwd)
+        if kind != "kl":
+            tri[kind] = (term[v].mean(), kl[v].mean(), kl[v].max())
+        g[kind] = _valid_bptt(flat, lanes, dims, cache, dmu, dls)
+    return tri, g
+
+
+class HostTarget(object):
+    """The get / set_param_values surface the host optimizers drive, over a float64 vector."""
+
+    def __init__(self, theta):
+        self.theta = np.array(theta, dtype=np.float64)
+
+    def get_param_values(self, trainable=False):
+        return self.theta.copy()
+
+    def set_param_values(self, v, trainable=False):
+        self.theta = np.array(v, dtype=np.float64)
+
+
+def lbfgs_step(optimizer, theta0, lanes, dims, kind, step_size=None, loss_kl=loss_kl, grad=grad):
+    """One optimize() of a host L-BFGS optimizer from theta0, driven by float64 callables of this oracle over lanes: a
+    PenaltyLbfgsOptimizer under the constraint mean KL <= step_size (PPO, penalty_lbfgs_optimizer.py over npo.py), or an
+    LbfgsOptimizer when step_size is None (ERWR, lbfgs_optimizer.py over vpg.py).  loss_kl / grad: the oracle of the
+    policy (categorical_gru_oracle passes its own).  Returns theta and the (loss, mean KL) pairs before and after."""
+    tgt = HostTarget(theta0)
+
+    def f_loss_kl(d):
+        return loss_kl(tgt.theta, d, dims, kind)
+
+    def f_opt(d, penalty=0.0):
+        loss, mkl, _ = f_loss_kl(d)
+        return loss + penalty * mkl, grad(tgt.theta, d, dims, kind, penalty=penalty)
+
+    def f_penalized_loss(d, penalty):
+        loss, mkl, _ = f_loss_kl(d)
+        return loss + penalty * mkl, loss, mkl
+
+    f_loss = lambda d: f_loss_kl(d)[0]
+    if step_size is None:
+        optimizer.update_opt(loss=f_loss, target=tgt, f_opt=f_opt)
+    else:
+        optimizer.update_opt(loss=f_loss, target=tgt, leq_constraint=(lambda d: f_loss_kl(d)[1], step_size), f_opt=f_opt,
+                             f_penalized_loss=f_penalized_loss)
+    before = f_loss_kl(lanes)[:2]
+    optimizer.optimize([lanes])
+    return tgt.theta, before, f_loss_kl(lanes)[:2]
 
 
 def tangent_mean(flat, lanes, dims, xvec):

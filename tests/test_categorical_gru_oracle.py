@@ -65,14 +65,16 @@ def test_loss_and_gradients_match_autograd(seed, masked, inc):
     dims, theta, lanes = _case(seed, masked, inc)
     th = torch.tensor(theta + 0.02 * np.random.RandomState(seed + 7).randn(dims.P), requires_grad=True)
     t = _torch_terms(th, lanes, dims)
+    tri, gs = C.pass_refs(th.detach().numpy(), lanes, dims)
     for kind in ("trpo", "vpg"):
         surr, kl, kl_max = C.loss_kl(th.detach().numpy(), lanes, dims, kind)
         np.testing.assert_allclose([surr, kl, kl_max], [t[kind].item(), t["kl"].item(), t["kl_max"].item()],
                                    rtol=0, atol=1e-12)
-        for penalty in (0.0, 0.5):
+        np.testing.assert_allclose(tri[kind], [surr, kl, kl_max], rtol=0, atol=1e-12)
+        for penalty in (0.0, 0.5, 1e3):
             g_ref = torch.autograd.grad(t[kind] + penalty * t["kl"], th, retain_graph=True)[0].numpy()
-            g = C.grad(th.detach().numpy(), lanes, dims, kind, penalty)
-            assert np.max(np.abs(g - g_ref)) <= 1e-10 * max(1.0, np.max(np.abs(g_ref)))
+            for g in (C.grad(th.detach().numpy(), lanes, dims, kind, penalty), gs[kind] + penalty * gs["kl"]):
+                assert np.max(np.abs(g - g_ref)) <= 1e-10 * max(1.0, np.max(np.abs(g_ref)))
     g_ref = torch.autograd.grad(t["kl"], th)[0].numpy()
     g = C.grad(th.detach().numpy(), lanes, dims, "kl")
     assert np.max(np.abs(g - g_ref)) <= 1e-10 * max(1.0, np.max(np.abs(g_ref)))

@@ -1,9 +1,9 @@
 """GPU: CategoricalGRUPolicy -- the fused recurrent discrete-action rollout and get_actions, the loss/KL, BPTT gradient
 (+ KL penalty) and Fisher-vector passes in float32, and the float64 parity passes, against the float64 oracle
 (tests/categorical_gru_oracle.py) on lanes whose paths restart mid-lane, masked and unmasked, for both values of
-state_include_action; saturated softmax probabilities; whole TRPO steps (float32, precision="f64",
-FiniteDifferenceHvp), VPG / PPO / ERWR through the host API, the rejections of CEM / REPS / sub-sampling, and the
-recurrent wire format on gym CartPole-v0."""
+state_include_action, at theta_old and away from it; saturated softmax probabilities; whole TRPO steps (float32,
+precision="f64", FiniteDifferenceHvp) and their accepted points, VPG, PPO and ERWR steps against the oracle-driven
+optimizers, the rejections of CEM / REPS / sub-sampling, and the recurrent wire format on gym CartPole-v0."""
 import os
 
 import numpy as np
@@ -15,11 +15,32 @@ pytestmark = pytest.mark.gpu
 import categorical_gru_oracle as C   # noqa: E402
 import categorical_oracle as CO      # noqa: E402
 
-# float32 BPTT error bound per T, relative to the largest entry of the float64 result: the largest error an H100 80GB
-# HBM3 measured over the passes, lane counts, mask settings and both input layouts of test_passes_match_oracle at that
-# T (DESIGN.md section 5: at most 9e-7 at every T outside the 20000-lane case), with a margin of about 4x; T = 16 keeps
-# the Gaussian GRU's bound for the 20000-lane case, whose penalised gradients sum the most samples.
+# The points the update passes are evaluated at: theta_old (ratio 1, KL 0); near, theta_old + 0.02 randn, what TRPO's
+# backtracking line search and the first L-BFGS iterates evaluate; far, the theta3 rule of test_gpu_update_shapes.py
+# (log p[a] - log q[a] of the taken actions spanning -2 .. 1), where PPO's penalty L-BFGS probes.
+POINTS = ("old", "near", "far")
+PENALTIES = (0.0, 1.0, 1e3)
+# float32 BPTT error bound per T, relative to the largest entry of the float64 result, at every point: the largest error
+# an H100 80GB HBM3 measured over the passes, lane counts, mask settings and both input layouts of
+# test_passes_match_oracle at that T with a margin of about 4x (DESIGN.md section 5): at most 9e-7 at every T and
+# point outside the 20000-lane case; T = 16 keeps the Gaussian GRU's bound for the 20000-lane case, whose penalised
+# gradients sum the most samples.
 F32_TOL = {1: 4e-6, 16: 2e-5, 100: 4e-6, 200: 4e-6}
+# the saturated heads of test_saturated_softmax (measured 4.1e-6 at theta_old, 1.5e-6 near it)
+SAT_TOL = 1e-4
+# penalty 1e3: the per-sample logit delta pen (p - q p / (p + TINY)) carries the float32 probabilities' rounding, about
+# one ulp of 1, so on top of the bound the gradient may err by PEN_FLOOR_K * pen ulp(1) (_grad_err); the largest error
+# measured was 0.10 of that term
+PEN_FLOOR_K = 0.4
+# relative bound of the float32 (loss, mean KL, max KL) triple over an absolute floor of 5e-7: the float32 KL near 0 is
+# a difference of two logs of nearly equal probabilities, ~1e-7 absolute (no excess over the floor measured)
+TRIPLE_RTOL = 1e-5
+# relative bound of the loss and mean KL TRPO records at its accepted parameters, float32 and float64 passes (measured
+# 2.2e-7 and 4.4e-16)
+ACCEPTED_RTOL = {"f32": 2e-6, "f64": 1e-12}
+# theta after one or two L-BFGS iterations of PPO / ERWR against the oracle-driven run (measured at most 9.2e-9; the
+# Gaussian GRU's bound)
+LBFGS_THETA_RTOL = 2.5e-7
 
 
 @pytest.fixture(scope="module")
@@ -49,6 +70,13 @@ def _f32(a):
 
 def _rel(a, b):
     return np.max(np.abs(a - b)) / np.max(np.abs(b))
+
+
+def _grad_err(g, ref, floor):
+    """The error of a float32 gradient relative to the largest oracle entry, less what an absolute floor (the rounding
+    a KL penalty amplifies) accounts for, and the error as a multiple of that floor."""
+    e = np.max(np.abs(g - ref))
+    return max(e - PEN_FLOOR_K * floor, 0.0) / np.max(np.abs(ref)), (e / floor if floor else 0.0)
 
 
 def _theta(dims, seed, scale=0.2):
@@ -190,37 +218,83 @@ def _lane_case(dev, dims, N, T, masked, seed, theta=None):
     return b, theta, lanes
 
 
-def _check_passes(dev, inc, b, theta, lanes, tol, tag, f64_only_rel=1e-10):
+def _eval_point(point, theta, lanes, dims, seed):
+    """The evaluation point of POINTS for lanes recorded at theta, rounded to float32 as the kernels read it."""
+    if point == "old":
+        return theta
+    if point == "near":
+        return _f32(theta + 0.02 * np.random.RandomState(seed).randn(dims.P))
+    # log p[a] - log q[a] cannot exceed -log q[a], and the q[a] of these lanes are mostly above e^-2: the upper end of
+    # the span is 1
+    v = C.GO.valid_of(lanes)
+    for s in range(10, 20):
+        d = np.random.RandomState(s).randn(dims.P)
+        for step in (0.1, 0.15, 0.2, 0.3, 0.5):
+            th = _f32(theta + d * step)
+            lr = C.log_ratio(th, lanes, dims)[v]
+            if lr.min() <= -2.0 and lr.max() >= 1.0:
+                return th
+    raise AssertionError("no far point spans the log likelihood ratios -2 .. 1")
+
+
+def _assert_triple(o, ref, point, what):
+    np.testing.assert_allclose(o, ref, rtol=TRIPLE_RTOL, atol=5e-7, err_msg="%s at %s" % (what, point))
+    return np.max(np.maximum(np.abs(o - ref) - 5e-7, 0.0) / np.abs(ref))
+
+
+def _check_passes(dev, inc, b, theta, lanes, tols, tag, f64_only_rel=1e-10, seed=0):
+    """At each point of tols (point -> float32 bound): the float32 loss/KL triple, gradient and penalised gradient
+    passes (the penalised pass's triple is the gradient pass's, bit for bit) and the float64 parity passes against the
+    oracle; the float64 KL gradient near theta_old; the Fisher product at theta_old only, the one point CG evaluates
+    it."""
     ops, L = _ops(), _L()
     dims, gd = _dims(inc)
-    th32 = torch.tensor(theta, dtype=torch.float32, device=dev)
-    th64 = torch.tensor(theta, dtype=torch.float64, device=dev)
     out = torch.empty(3, dtype=torch.float64, device=dev)
-    g = torch.empty(dims.P, dtype=torch.float64, device=dev)
-    errs = {}
-    for kind, lk in (("trpo", L.LOSS_TRPO), ("vpg", L.LOSS_VPG)):
-        ref = np.array(C.loss_kl(theta, lanes, dims, kind))
-        ops.loss_kl(lk, th32, gd, None, b, out)
-        # atol: the float32 KL near 0 is a difference of two logs of nearly equal probabilities, ~1e-7 absolute
-        np.testing.assert_allclose(out.cpu().numpy(), ref, rtol=1e-5, atol=5e-7)
-        ops.update_f64(0, lk, th64, gd, None, b, None, 0.0, 0.0, None, out)
-        np.testing.assert_allclose(out.cpu().numpy(), ref, rtol=1e-10, atol=1e-13)
-        for pen in (0.0, 0.5):
-            gref = C.grad(theta, lanes, dims, kind, penalty=pen)
-            if pen:
-                ops.grad_penalized(lk, pen, th32, gd, None, b, g, out)
-            else:
-                ops.grad(lk, th32, gd, None, b, g, out)
-            assert np.all(np.isfinite(g.cpu().numpy()))
-            errs["grad_%s_%g" % (kind, pen)] = _rel(g.cpu().numpy(), gref)
-        gref = C.grad(theta, lanes, dims, kind)
-        ops.update_f64(1, lk, th64, gd, None, b, None, 0.0, 0.0, g, out)
-        np.testing.assert_allclose(g.cpu().numpy(), gref, rtol=0, atol=f64_only_rel * np.abs(gref).max())
+    tri0, tri = (torch.empty(3, dtype=torch.float64, device=dev) for _ in range(2))
+    g0, g = (torch.empty(dims.P, dtype=torch.float64, device=dev) for _ in range(2))
+    for point, tol in tols.items():
+        th = _eval_point(point, theta, lanes, dims, seed)
+        tri_ref, g_ref = C.pass_refs(th, lanes, dims)
+        if point == "far":
+            assert tri_ref["trpo"][1] > 1e-3
+        th32 = torch.tensor(th, dtype=torch.float32, device=dev)
+        th64 = torch.tensor(th, dtype=torch.float64, device=dev)
+        errs, terr, fl = {}, {}, {}
+        for kind, lk in (("trpo", L.LOSS_TRPO), ("vpg", L.LOSS_VPG)):
+            ref = np.array(tri_ref[kind])
+            ops.loss_kl(lk, th32, gd, None, b, out)
+            terr["loss_pass_" + kind] = _assert_triple(out.cpu().numpy(), ref, point, "loss pass " + kind)
+            ops.update_f64(0, lk, th64, gd, None, b, None, 0.0, 0.0, None, out)
+            np.testing.assert_allclose(out.cpu().numpy(), ref, rtol=1e-10, atol=1e-13)
+            ops.grad(lk, th32, gd, None, b, g0, tri0)
+            terr["grad_pass_" + kind] = _assert_triple(tri0.cpu().numpy(), ref, point, "gradient pass " + kind)
+            for pen in PENALTIES:
+                gref = g_ref[kind] + pen * g_ref["kl"]
+                if pen:
+                    ops.grad_penalized(lk, pen, th32, gd, None, b, g, tri)
+                    assert torch.equal(tri, tri0)
+                else:
+                    g.copy_(g0)
+                assert np.all(np.isfinite(g.cpu().numpy()))
+                key = "grad_%s_%g" % (kind, pen)
+                floor = pen * float(np.spacing(np.float32(1.0))) if pen >= 1e3 else 0.0
+                errs[key], efl = _grad_err(g.cpu().numpy(), gref, floor)
+                if floor:
+                    fl[key] = efl
+                assert errs[key] < tol, (point, key, errs[key], efl)
+            gref = g_ref[kind]
+            ops.update_f64(1, lk, th64, gd, None, b, None, 0.0, 0.0, g, out)
+            np.testing.assert_allclose(g.cpu().numpy(), gref, rtol=0, atol=f64_only_rel * np.abs(gref).max())
+        print("categorical GRU float32 error %s point=%s: %s | of the penalty floor %s | triple %s" % (
+            tag, point, " ".join("%s=%.2e" % kv for kv in sorted(errs.items())),
+            " ".join("%s=%.2e" % kv for kv in sorted(fl.items())), " ".join("%s=%.2e" % kv for kv in sorted(terr.items()))))
     th_kl = theta + 1e-3 * np.random.RandomState(7).randn(dims.P)
     gk = C.grad(th_kl, lanes, dims, "kl")
     ops.update_f64(1, L.LOSS_KL, torch.tensor(th_kl, device=dev), gd, None, b, None, 0.0, 0.0, g, None)
     np.testing.assert_allclose(g.cpu().numpy(), gk, rtol=0, atol=f64_only_rel * np.abs(gk).max())
     # Fisher product at theta_old: old_prob = the policy's own float32 probabilities
+    th32 = torch.tensor(theta, dtype=torch.float32, device=dev)
+    th64 = torch.tensor(theta, dtype=torch.float64, device=dev)
     p32 = np.moveaxis(C.forward(theta, lanes, dims)[0], -1, 0).astype(np.float32)
     b.mean.copy_(torch.tensor(p32))
     lanes = dict(lanes, old_prob=p32)
@@ -228,7 +302,7 @@ def _check_passes(dev, inc, b, theta, lanes, tol, tag, f64_only_rel=1e-10):
     ref = C.fvp(theta, lanes, dims, x.cpu().numpy(), 1e-5)
     hx = torch.empty_like(x)
     ops.fvp(th32, gd, None, b, x, 1e-5, 1.0, hx)
-    errs["fvp"] = _rel(hx.cpu().numpy(), ref)
+    err = _rel(hx.cpu().numpy(), ref)
     hc = b.hcache(32, 0)
     ops.grad(L.LOSS_TRPO, th32, gd, None, b, g, out, hc)
     hx2 = torch.empty_like(x)
@@ -236,8 +310,8 @@ def _check_passes(dev, inc, b, theta, lanes, tol, tag, f64_only_rel=1e-10):
     np.testing.assert_array_equal(hx2.cpu().numpy(), hx.cpu().numpy())
     ops.update_f64(2, L.LOSS_TRPO, th64, gd, None, b, x, 1e-5, 1.0, hx, None)
     np.testing.assert_allclose(hx.cpu().numpy(), ref, rtol=0, atol=f64_only_rel * np.abs(ref).max())
-    print("categorical GRU float32 error %s: %s" % (tag, " ".join("%s=%.2e" % kv for kv in sorted(errs.items()))))
-    assert max(errs.values()) < tol, errs
+    print("categorical GRU float32 error %s: fvp=%.2e" % (tag, err))
+    assert err < tols["old"], err
 
 
 # 20000 lanes are 157 tiles of 128: more than one tile per CTA of the gradient pass on 132 SMs
@@ -247,14 +321,16 @@ def _check_passes(dev, inc, b, theta, lanes, tol, tag, f64_only_rel=1e-10):
 def test_passes_match_oracle(dev, T, N, masked, inc):
     dims, _ = _dims(inc)
     b, theta, lanes = _lane_case(dev, dims, N, T, masked, 10 + T + int(masked))
-    _check_passes(dev, inc, b, theta, lanes, F32_TOL[T], "T=%d N=%d masked=%s inc=%s" % (T, N, masked, inc))
+    _check_passes(dev, inc, b, theta, lanes, {p: F32_TOL[T] for p in POINTS},
+                  "T=%d N=%d masked=%s inc=%s" % (T, N, masked, inc), seed=T)
 
 
 @pytest.mark.parametrize("gap", [8.0, 17.0, 40.0])
 @pytest.mark.parametrize("sign", [1.0, -1.0])
 def test_saturated_softmax(dev, gap, sign):
-    """Probabilities within ~1e-7 of 0 or 1 (logit gaps 17 and 40) give finite passes that agree with the oracle: the
-    output bias sets the gap, and W_out is scaled so that h moves it by at most 0.25."""
+    """Probabilities within ~1e-7 of 0 or 1 (logit gaps 17 and 40) give finite passes that agree with the oracle, at
+    theta_old and near it, where q of the unlikely action (~1e-7 .. 1e-17) makes the TINY terms of the KL and of its
+    logit gradient matter: the output bias sets the gap, and W_out is scaled so that h moves it by at most 0.25."""
     inc = True
     dims, _ = _dims(inc)
     rng = np.random.RandomState(int(gap))
@@ -266,7 +342,7 @@ def test_saturated_softmax(dev, gap, sign):
     theta[-2:] = sign * 0.5 * gap * np.array([1.0, -1.0])
     theta = _f32(theta)
     b, theta, lanes = _lane_case(dev, dims, 300, 16, True, 3, theta)
-    _check_passes(dev, inc, b, theta, lanes, 1e-4, "gap=%g sign=%g" % (gap, sign), f64_only_rel=1e-9)
+    _check_passes(dev, inc, b, theta, lanes, {"old": SAT_TOL, "near": SAT_TOL}, "gap=%g sign=%g" % (gap, sign), f64_only_rel=1e-9, seed=int(gap))
 
 
 def test_gradient_pass_ignores_stale_cache(dev):
@@ -326,11 +402,21 @@ def test_trpo_step_matches_oracle(dev, precision, tol):
     theta0 = algo.policy.theta32.double().cpu().numpy() if precision == "f32" else theta0
     algo.optimize_policy(0, sd)
     theta_dev = algo.policy.get_param_values()
-    theta_ref, info = C.trpo_step(theta0, lanes, C.CatGruDims(4, 32, 2, True), 0.01, 4)
+    dims = C.CatGruDims(4, 32, 2, True)
+    theta_ref, info = C.trpo_step(theta0, lanes, dims, 0.01, 4)
     li = algo.optimizer.last_info
     assert not li["rejected"] and not info["rejected"] and li["n_iter"] == info["n_iter"]
     assert _rel(theta_dev - theta0, theta_ref - theta0) < tol, _rel(theta_dev - theta0, theta_ref - theta0)
     assert 0 < li["constraint_val"] <= 0.01
+    # the line search's loss pass off theta_old: the loss and mean KL recorded at the accepted parameters (as the
+    # kernels read them) are the oracle's there
+    th_acc = algo.policy.theta32.double().cpu().numpy() if precision == "f32" else theta_dev
+    loss, mkl, _ = C.loss_kl(th_acc, lanes, dims, "trpo")
+    print("categorical GRU TRPO %s accepted point: loss %.3e rel err %.2e, mean KL %.3e rel err %.2e" % (
+        precision, loss, abs(li["loss"] / loss - 1), mkl, abs(li["constraint_val"] / mkl - 1)))
+    rtol = ACCEPTED_RTOL[precision]
+    np.testing.assert_allclose(li["loss"], loss, rtol=rtol, atol=1e-7 if precision == "f32" else 1e-13)
+    np.testing.assert_allclose(li["constraint_val"], mkl, rtol=rtol)
 
 
 def test_trpo_finite_difference_hvp(dev):
@@ -347,6 +433,92 @@ def test_trpo_finite_difference_hvp(dev):
     assert not li["rejected"] and 0 < li["constraint_val"] <= 0.01
     d = algo.policy.get_param_values() - theta0
     assert _rel(d, theta_ref - theta0) < 2e-2, _rel(d, theta_ref - theta0)
+
+
+@pytest.mark.parametrize("inc", [True, False])
+def test_vpg_updates_match_oracle(dev, inc):
+    """Three VPG iterations (Adam moments and step counter carried): theta after each device Adam step is the oracle's
+    Adam step on the oracle gradient at float32(theta), and the after-step (loss, mean KL, max KL), off theta_old, is the
+    oracle's at the device's new parameters; each iteration restarts from the oracle's theta."""
+    from oracle import policy as P
+    dims, _ = _dims(inc)
+    algo = _algo("vpg", inc=inc)
+    algo.start_worker()
+    algo.init_opt()
+    adam = (np.zeros(dims.P), np.zeros(dims.P), 0)
+    for itr in range(3):
+        sd = algo.sampler.process_samples(itr, algo.sampler.obtain_samples(itr))
+        lanes = _oracle_lanes(sd)
+        theta0 = algo.policy.get_param_values()
+        g_ref = C.grad(algo.policy.theta32.double().cpu().numpy(), lanes, dims, "vpg")
+        theta_ref, m, v, t = P.adam_step(theta0, g_ref, *adam)
+        adam = (m, v, t)
+        algo.optimize_policy(itr, sd)
+        after = np.array([algo.optimizer.eval_lazy(sd)[i] for i in range(3)])    # LossAfter, MeanKL, MaxKL
+        ref = np.array(C.loss_kl(algo.policy.theta32.double().cpu().numpy(), lanes, dims, "vpg"))
+        rel = _rel(algo.policy.get_param_values(), theta_ref)
+        print("categorical GRU VPG inc=%s itr %d: theta rel err %.2e, after-step triple %s vs oracle %s" %
+              (inc, itr, rel, after, ref))
+        assert rel < 1e-5, (itr, rel)
+        assert ref[1] > 0
+        np.testing.assert_allclose(after, ref, rtol=TRIPLE_RTOL, atol=5e-7)
+        algo.policy.set_param_values(theta_ref)     # keep both sides on the same trajectory of parameters
+
+
+def _lbfgs_steps(name, optimizer_args):
+    """One PPO (kind trpo, KL <= 0.01) or ERWR (kind vpg, shifted advantages) policy update on the device, and the same
+    host optimizer driven by the oracle over the read-back lanes from the same theta."""
+    from rllab_b200.optimizers.lbfgs_optimizer import LbfgsOptimizer
+    from rllab_b200.optimizers.penalty_lbfgs_optimizer import PenaltyLbfgsOptimizer
+    dims, _ = _dims(True)
+    algo = _algo(name, optimizer_args=optimizer_args)
+    algo.start_worker()
+    algo.init_opt()
+    sd = algo.sampler.process_samples(0, algo.sampler.obtain_samples(0))
+    lanes = _oracle_lanes(sd)
+    theta0 = algo.policy.get_param_values()
+    before = algo._objective.eval_lazy(sd)[0]
+    algo.optimize_policy(0, sd)
+    after = (algo._objective.eval_lazy(sd)[0], algo._objective.eval_lazy(sd)[1])
+    if name == "ppo":
+        opt = PenaltyLbfgsOptimizer(**optimizer_args)
+        th_ref, before_ref, after_ref = C.lbfgs_step(opt, theta0, lanes, dims, "trpo", step_size=0.01)
+    else:
+        opt = LbfgsOptimizer(**optimizer_args)
+        th_ref, before_ref, after_ref = C.lbfgs_step(opt, theta0, lanes, dims, "vpg")
+    th = algo.policy.get_param_values()
+    rel = np.max(np.abs(th - th_ref)) / np.max(np.abs(th_ref))
+    print("categorical GRU %s %s: penalties %s vs oracle %s; theta rel err %.2e; loss %.6g -> %.6g (oracle %.6g -> "
+          "%.6g), kl %.4g (oracle %.4g)" % (name, optimizer_args, getattr(algo.optimizer, "tried_penalties", None),
+                                            getattr(opt, "tried_penalties", None), rel, before, after[0],
+                                            before_ref[0], after_ref[0], after[1], after_ref[1]))
+    return algo, opt, theta0, th, th_ref, rel, (before, after), (before_ref, after_ref)
+
+
+@pytest.mark.parametrize("max_opt_itr", [1, 2])
+def test_ppo_step_short_matches_oracle(dev, max_opt_itr):
+    """max_opt_itr 1 / 2: the same penalties tried as the oracle-driven PenaltyLbfgsOptimizer, theta close to its."""
+    algo, opt, _, _, _, rel, _, _ = _lbfgs_steps("ppo", dict(max_opt_itr=max_opt_itr))
+    assert algo.optimizer.tried_penalties == opt.tried_penalties
+    assert rel < LBFGS_THETA_RTOL, rel
+
+
+def test_ppo_step_defaults(dev):
+    """Default settings: the loss decreases, the accept decision (theta moved or restored) is the oracle's, and the mean
+    KL is within the step size whenever the oracle's is."""
+    _, _, theta0, th, th_ref, _, (before, after), (_, after_ref) = _lbfgs_steps("ppo", dict())
+    assert after[0] < before
+    assert np.array_equal(th, theta0) == np.array_equal(th_ref, theta0)
+    if after_ref[1] <= 0.01:
+        assert after[1] <= 0.01
+
+
+@pytest.mark.parametrize("max_opt_itr", [1, 2])
+def test_erwr_step_matches_oracle(dev, max_opt_itr):
+    """ERWR's LbfgsOptimizer on the VPG surrogate of the shifted (non-negative) advantages, max_opt_itr 1 / 2: theta
+    close to the oracle-driven run's."""
+    _, _, _, _, _, rel, _, _ = _lbfgs_steps("erwr", dict(max_opt_itr=max_opt_itr))
+    assert rel < LBFGS_THETA_RTOL, rel
 
 
 @pytest.mark.parametrize("name", ["vpg", "ppo", "erwr"])

@@ -1,6 +1,6 @@
 """CPU: the float64 GRU oracle (tests/gru_oracle.py) against torch.autograd in float64 -- loss/KL, the BPTT gradients
-(surrogate, KL, KL-penalised) and the Fisher-vector product by double backward -- on lanes whose paths restart mid-lane,
-with and without masked paths; its forward against torch.nn.GRU; and the host-side GaussianGRUPolicy surface."""
+(surrogate, KL, KL-penalised with penalties up to 1e3) at theta_old and away from it, and the Fisher-vector product by
+double backward -- on lanes whose paths restart mid-lane, with and without masked paths; its forward against torch.nn.GRU; and the host-side GaussianGRUPolicy surface."""
 import numpy as np
 import pytest
 
@@ -64,18 +64,35 @@ def _torch_terms(th, lanes, dims, old_mean=None):
 @pytest.mark.parametrize("masked", [False, True])
 @pytest.mark.parametrize("inc", [True, False])
 def test_loss_and_gradients_match_autograd(masked, inc):
-    dims, theta, lanes = _case(1 + int(masked) + 2 * int(inc), masked, inc)
-    th = torch.tensor(theta, requires_grad=True)
-    trpo, vpg, mkl, xkl = _torch_terms(th, lanes, dims)
-    for kind, ref in (("trpo", trpo), ("vpg", vpg)):
-        lo = G.loss_kl(theta, lanes, dims, kind)
-        np.testing.assert_allclose(lo, [ref.item(), mkl.item(), xkl.item()], rtol=1e-12, atol=1e-14)
-        g_ref = torch.autograd.grad(ref, th, retain_graph=True)[0].numpy()
-        np.testing.assert_allclose(G.grad(theta, lanes, dims, kind), g_ref, rtol=1e-10, atol=1e-13)
-        gp_ref = torch.autograd.grad(ref + 0.7 * mkl, th, retain_graph=True)[0].numpy()
-        np.testing.assert_allclose(G.grad(theta, lanes, dims, kind, penalty=0.7), gp_ref, rtol=1e-10, atol=1e-13)
-    gk_ref = torch.autograd.grad(mkl, th)[0].numpy()
-    np.testing.assert_allclose(G.grad(theta, lanes, dims, "kl"), gk_ref, rtol=1e-10, atol=1e-13)
+    """At theta_old (ratio 1, KL 0, a zero KL-penalty gradient) and at theta_old + 0.15 randn with log_std moved by 0.3,
+    where the ratio, every KL term and the penalty gradients are away from their trivial values."""
+    dims, theta_old, lanes = _case(1 + int(masked) + 2 * int(inc), masked, inc)
+    moved = theta_old + 0.15 * np.random.RandomState(5).randn(dims.P)
+    moved[-dims.A:] += 0.3
+    for theta in (theta_old, moved):
+        th = torch.tensor(theta, requires_grad=True)
+        trpo, vpg, mkl, xkl = _torch_terms(th, lanes, dims)
+        if theta is moved:
+            assert mkl.item() > 1e-3
+        tri, gs = G.pass_refs(theta, lanes, dims)
+        for kind, ref in (("trpo", trpo), ("vpg", vpg)):
+            lo = G.loss_kl(theta, lanes, dims, kind)
+            np.testing.assert_allclose(lo, [ref.item(), mkl.item(), xkl.item()], rtol=1e-12, atol=1e-14)
+            np.testing.assert_allclose(tri[kind], lo, rtol=1e-12, atol=1e-14)
+            g_ref = torch.autograd.grad(ref, th, retain_graph=True)[0].numpy()
+            np.testing.assert_allclose(G.grad(theta, lanes, dims, kind), g_ref, rtol=1e-10, atol=1e-13)
+            for pen in (0.7, 1.0, 1e3):
+                gp_ref = torch.autograd.grad(ref + pen * mkl, th, retain_graph=True)[0].numpy()
+                np.testing.assert_allclose(G.grad(theta, lanes, dims, kind, penalty=pen), gp_ref, rtol=1e-10,
+                                           atol=1e-13)
+                np.testing.assert_allclose(gs[kind] + pen * gs["kl"], gp_ref, rtol=1e-10, atol=1e-13)
+        gk_ref = torch.autograd.grad(mkl, th)[0].numpy()
+        np.testing.assert_allclose(G.grad(theta, lanes, dims, "kl"), gk_ref, rtol=1e-10, atol=1e-13)
+        # the per-sample log likelihood ratio the far evaluation points of the GPU tests are chosen by
+        lr = torch.log(_torch_terms(th, dict(lanes, adv=np.full(lanes["adv"].shape, -1.0)), dims)[0])
+        v = G.valid_of(lanes)
+        np.testing.assert_allclose(np.log(np.exp(G.log_ratio(theta, lanes, dims)[v]).mean()), lr.item(), rtol=1e-12,
+                                   atol=1e-14)
 
 
 @pytest.mark.parametrize("masked", [False, True])
